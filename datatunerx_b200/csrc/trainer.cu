@@ -9,8 +9,10 @@
 // GEMM serves each pair; LoRA masters fp32 in one flat buffer (A^T[d,r] | B[d,r] per target per layer) with
 // m, v and the gradient in identically laid-out flat buffers (one NCCL all-reduce, one AdamW launch);
 // bf16 "shadows" of the adapters padded to a 64-wide rank block feed the tensor-core GEMMs.
-// Activations needed by backward are kept (no recompute: 180 GB HBM makes gradient checkpointing pointless
-// for 7B LoRA at 16K tokens/step).
+// Activations needed by backward are kept per layer when they fit in device memory (7B LoRA at 8K tokens/step: 43 GB of
+// 80); otherwise one shared set of decoder-layer activations is refilled by re-running each layer's forward in the backward
+// pass (gradient checkpointing per layer, DESIGN.md §3).  Both layouts launch the same kernels on the same inputs, so they
+// give bitwise-identical results.
 #include "kernels.h"
 #include "../../include/dtxtune.h"
 
@@ -156,6 +158,14 @@ struct Layer {
   float* absmax[4] = {nullptr, nullptr, nullptr, nullptr};
 };
 enum { W_QKV = 0, W_O = 1, W_GU = 2, W_DOWN = 3 };
+// activation layouts (dtx_train_cfg.recompute): every layer keeps its own saved set, or all layers share one that the
+// backward pass refills by re-running each layer's forward
+enum { KEEP_ALL = 1, RECOMPUTE_LAYER = 2 };
+// which part of the step asks for a base weight (the NF4 prefetch predicts the next one from it)
+enum { PH_FWD = 0, PH_RECOMPUTE = 1, PH_BWD = 2 };
+// automatic layout choice: what the trainer may not take of the free device memory (NCCL communicator buffers, created
+// after the trainer's own, and cudaMalloc granularity)
+constexpr int64_t kHeadroomBytes = int64_t(1) << 30;
 
 }  // namespace
 void trainer_set_fused_epilogues(int on) { g_fused_epilogues = on; }
@@ -177,6 +187,8 @@ struct dtx_trainer {
   std::string err;
   std::vector<void*> allocs;
   size_t bytes_allocated = 0;
+  bool dry = false;             // sizing only (dtx_plan_device_bytes, automatic layout): alloc() counts bytes, nothing is allocated
+  int recompute = KEEP_ALL;     // activation layout in use
 
   int M = 0, RP = 0, nt = 0;    // M = micro_batch * seq_len: the largest batch this trainer was created for
   int cur_S = 0, cur_M = 0;     // padded length / token count of the batch being processed (<= seq_len / M)
@@ -271,6 +283,11 @@ struct dtx_trainer {
   }
   template <typename T>
   bool alloc(T** p, size_t n) {
+    if (dry) {
+      bytes_allocated += n * sizeof(T);
+      *p = nullptr;
+      return true;
+    }
     void* q = nullptr;
     cudaError_t e = cudaMalloc(&q, n * sizeof(T));
     if (e != cudaSuccess) {
@@ -293,6 +310,11 @@ struct dtx_trainer {
       }
     cudaFree(p);
     bytes_allocated -= bytes;
+  }
+  // cudaMemset of a buffer create_buffers() just allocated (nothing in a sizing run)
+  template <typename T>
+  cudaError_t zero(T* p, size_t n) {
+    return dry ? cudaSuccess : cudaMemset(p, 0, n * sizeof(T));
   }
   // first base tensor that has not been loaded, or nullptr when the model is complete
   const char* missing_weight(char* buf, size_t n) const {
@@ -347,8 +369,8 @@ uint64_t dropout_key(const dtx_trainer* t, int layer) {
   return x ^ (x >> 31);
 }
 
-int pick_split(int m_tiles, int kb_total) {
-  int s = (2 * gemm_num_sms() + m_tiles - 1) / m_tiles;
+int pick_split(int n_sms, int m_tiles, int kb_total) {
+  int s = (2 * n_sms + m_tiles - 1) / m_tiles;
   if (s < 1) s = 1;
   if (s > 16) s = 16;
   if (s > kb_total) s = kb_total;
@@ -383,10 +405,10 @@ int create_buffers(dtx_trainer* t) {
     ok = ok && t->alloc(&t->master, shard) && t->alloc(&t->fm, shard) && t->alloc(&t->fv, shard);
     ok = ok && t->alloc(&t->embed_g32, V * d) && t->alloc(&t->ndw_scratch, 64 * d);
     if (!ok) return DTX_ERR_CUDA;
-    CKM(cudaMemset(t->w_flat, 0, total * sizeof(bf16)));
-    CKM(cudaMemset(t->g_flat, 0, total * sizeof(bf16)));
-    CKM(cudaMemset(t->fm, 0, shard * sizeof(float)));
-    CKM(cudaMemset(t->fv, 0, shard * sizeof(float)));
+    CKM(t->zero(t->w_flat, total));
+    CKM(t->zero(t->g_flat, total));
+    CKM(t->zero(t->fm, shard));
+    CKM(t->zero(t->fv, shard));
     bf16* gl = t->w_flat + L * t->layer_elems;
     t->embed = gl;
     t->lm_head = gl + t->goff_lm;
@@ -396,8 +418,8 @@ int create_buffers(dtx_trainer* t) {
     ok = ok && t->alloc(&t->embed, V * d) && t->alloc(&t->lm_head, V * d) && t->alloc(&t->normf, d);
     ok = ok && t->alloc(&t->a_cat_all, L * RP * KA) && t->alloc(&t->b_ext_all, L * W * RP);
     if (!ok) return DTX_ERR_CUDA;
-    CKM(cudaMemset(t->a_cat_all, 0, L * RP * KA * sizeof(bf16)));
-    CKM(cudaMemset(t->b_ext_all, 0, L * W * RP * sizeof(bf16)));
+    CKM(t->zero(t->a_cat_all, L * RP * KA));
+    CKM(t->zero(t->b_ext_all, L * W * RP));
   }
   t->base_bytes = static_cast<int64_t>((2 * V * d + d) * sizeof(bf16));
   t->loaded.assign(3 + 9 * L, 0);
@@ -415,9 +437,15 @@ int create_buffers(dtx_trainer* t) {
            t->alloc(&y.wdown, d * F) && t->alloc(&y.norm1, d) && t->alloc(&y.norm2, d);
       y.a_cat = t->a_cat_all + l * RP * KA;
       y.b_ext = t->b_ext_all + l * W * RP;
-      ok = ok && t->alloc(&y.t, M * RP);
     }
     t->base_bytes += static_cast<int64_t>((W * d + d * d + 3 * F * d + 2 * d) * sizeof(bf16));
+    if (t->recompute == RECOMPUTE_LAYER && l > 0) {  // one saved set, refilled layer by layer
+      const Layer& y0 = t->layers[0];
+      y.h1 = y0.h1; y.t = y0.t; y.hd = y0.hd; y.qkv = y0.qkv; y.attn = y0.attn; y.x_mid = y0.x_mid; y.gu = y0.gu;
+      y.lse = y0.lse; y.rstd1 = y0.rstd1; y.rstd2 = y0.rstd2;
+      continue;
+    }
+    if (!full) ok = ok && t->alloc(&y.t, M * RP);
     ok = ok && t->alloc(&y.h1, M * d) && t->alloc(&y.qkv, M * W) &&
          t->alloc(&y.attn, M * d) && t->alloc(&y.x_mid, M * d) && t->alloc(&y.gu, M * 2 * F);
     if (t->dropout) ok = ok && t->alloc(&y.hd, M * KA);
@@ -429,10 +457,10 @@ int create_buffers(dtx_trainer* t) {
     ok = ok && t->alloc(&t->params, t->n_train) && t->alloc(&t->grads, t->n_train) && t->alloc(&t->adam_m, t->n_train) &&
          t->alloc(&t->adam_v, t->n_train);
     if (!ok) return DTX_ERR_CUDA;
-    CKM(cudaMemset(t->params, 0, t->n_train * sizeof(float)));
-    CKM(cudaMemset(t->grads, 0, t->n_train * sizeof(float)));
-    CKM(cudaMemset(t->adam_m, 0, t->n_train * sizeof(float)));
-    CKM(cudaMemset(t->adam_v, 0, t->n_train * sizeof(float)));
+    CKM(t->zero(t->params, t->n_train));
+    CKM(t->zero(t->grads, t->n_train));
+    CKM(t->zero(t->adam_m, t->n_train));
+    CKM(t->zero(t->adam_v, t->n_train));
   }
   ok = ok && t->alloc(&t->h2, M * d) && t->alloc(&t->act, M * F) && t->alloc(&t->dact, M * F) && t->alloc(&t->dgu, M * 2 * F) &&
        t->alloc(&t->dx_a, M * d) && t->alloc(&t->dx_b, M * d) && t->alloc(&t->dh, M * d) && t->alloc(&t->dattn, M * d) &&
@@ -440,8 +468,8 @@ int create_buffers(dtx_trainer* t) {
        t->alloc(&t->rstdf, M) && t->alloc(&t->row_loss, M) &&
        t->alloc(&t->delta, static_cast<size_t>(tc.micro_batch) * mc.n_heads * tc.seq_len);
   const int kb_tok = (static_cast<int>(M) + 63) / 64;
-  t->split_b = pick_split((static_cast<int>(W) + 127) / 128, kb_tok);
-  t->split_a = pick_split((static_cast<int>(KA) + 127) / 128, kb_tok);
+  t->split_b = pick_split(t->n_sms, (static_cast<int>(W) + 127) / 128, kb_tok);
+  t->split_a = pick_split(t->n_sms, (static_cast<int>(KA) + 127) / 128, kb_tok);
   if (!full)
     ok = ok && t->alloc(&t->part_b, static_cast<size_t>(t->split_b) * W * RP) &&
          t->alloc(&t->part_a, static_cast<size_t>(t->split_a) * KA * RP);
@@ -456,6 +484,7 @@ int create_buffers(dtx_trainer* t) {
   ok = ok && t->alloc(&t->rope_cs, static_cast<size_t>(tc.seq_len) * (mc.head_dim / 2));
   ok = ok && t->alloc(&t->rope_cs_t, static_cast<size_t>(tc.seq_len) * (mc.head_dim / 2));
   if (!ok) return DTX_ERR_CUDA;
+  if (t->dry) return DTX_OK;
   // rotary table in double precision (HF LlamaRotaryEmbedding: inv_freq = theta^(-2i/D))
   {
     const int half = mc.head_dim / 2;
@@ -514,24 +543,34 @@ int nf4_expand(dtx_trainer* t, int l, int which, cudaStream_t s) {
   CK(nf4_dequant_bf16(y.q4[which], y.absmax[which], t->scratch_w[which], n[which], s), 1);
   return DTX_OK;
 }
-// next (layer, matrix) the step will ask for after (l, which); backward = the step is in (or about to enter) its backward pass
-bool next_weight(const dtx_trainer* t, int l, int which, bool backward, bool will_backward, int* nl, int* nw) {
+// next (layer, matrix) the step will ask for after (l, which) in `phase` (PH_*), when it can be expanded ahead: always a
+// different matrix type than `which`, whose scratch the GEMM about to be launched reads.  A wrong guess is not merely slow:
+// the main stream would expand the mismatched matrix inline while the side stream may still be writing the same scratch.
+bool next_weight(const dtx_trainer* t, int l, int which, int phase, bool will_backward, int* nl, int* nw) {
   const int L = t->mc.n_layers;
-  if (!backward) {  // forward order: qkv, o, gu, down
+  if (phase == PH_FWD) {  // forward order: qkv, o, gu, down
     if (which < W_DOWN) { *nl = l; *nw = which + 1; return true; }
     if (l + 1 < L) { *nl = l + 1; *nw = W_QKV; return true; }
     if (will_backward) { *nl = L - 1; *nw = W_DOWN; return true; }
     return false;
+  }
+  if (phase == PH_RECOMPUTE) {  // qkv, o, gu (the down-projection is not re-run), then the same layer's backward
+    *nl = l;
+    *nw = which < W_GU ? which + 1 : W_DOWN;
+    return true;
   }
   // backward order: down, gu, o, qkv (layer 0's qkv is never asked for: no consumer of its input gradient)
   if (which > W_QKV) {
     if (which - 1 == W_QKV && l == 0) return false;
     *nl = l; *nw = which - 1; return true;
   }
+  // With per-layer recompute the layer below starts with its own q|k|v GEMM: the scratch the GEMM about to be launched reads
+  // (the prefetch is issued before that launch), so it cannot be expanded ahead; base_weight expands it inline behind that GEMM.
+  if (t->recompute == RECOMPUTE_LAYER) return false;
   if (l - 1 >= 0) { *nl = l - 1; *nw = W_DOWN; return true; }
   return false;
 }
-int base_weight(dtx_trainer* t, int l, int which, bool backward, bool will_backward, const bf16** out) {
+int base_weight(dtx_trainer* t, int l, int which, int phase, bool will_backward, const bf16** out) {
   Layer& y = t->layers[l];
   bf16* res[4] = {y.wqkv, y.wo, y.wgu, y.wdown};
   if (!t->quant4) {
@@ -548,7 +587,7 @@ int base_weight(dtx_trainer* t, int l, int which, bool backward, bool will_backw
   t->deq_layer[which] = l;
   *out = t->scratch_w[which];
   int nl, nw;
-  if (t->copy_stream && next_weight(t, l, which, backward, will_backward, &nl, &nw) && t->deq_layer[nw] != nl) {
+  if (t->copy_stream && next_weight(t, l, which, phase, will_backward, &nl, &nw) && t->deq_layer[nw] != nl) {
     // the scratch of type nw was last read by a GEMM launched earlier on the main stream: order the overwrite behind it
     CKM(cudaEventRecord(t->ev_scr[nw], t->stream));
     CKM(cudaStreamWaitEvent(t->copy_stream, t->ev_scr[nw], 0));
@@ -563,7 +602,7 @@ int base_weight(dtx_trainer* t, int l, int which, bool backward, bool will_backw
 #define BASEW(which, ptr)                                                        \
   const bf16* ptr = nullptr;                                                     \
   do {                                                                           \
-    int _rc = base_weight(t, l, which, in_backward, backward, &ptr);             \
+    int _rc = base_weight(t, l, which, phase, backward, &ptr);                   \
     if (_rc) return _rc;                                                         \
   } while (0)
 
@@ -595,6 +634,93 @@ int reduce_scatter_block(dtx_trainer* t, bf16* block, int64_t elems, int ev_idx)
   return DTX_OK;
 }
 
+// RoPE / SwiGLU run in the GEMM and attention epilogues: the switch is on and the batch fills whole 256-column tiles
+bool use_fused(const dtx_trainer* t) {
+  return g_fused_epilogues && t->cur_M > 128 && ((t->dq + t->dkv) % 256 == 0) && (t->W % 256 == 0);
+}
+
+// Forward of decoder layer l from xs[l]: fills the layer's saved activations (h1, hd, t, qkv, attn, lse, rstd1, x_mid, rstd2, gu)
+// and, in the forward pass proper (phase PH_FWD), xs[l + 1].  The per-layer recompute of the backward pass (PH_RECOMPUTE) runs
+// the very same launches - same epilogues, unfused fallbacks, packed / ragged arguments and dropout key (fwd_count is not
+// advanced) - so that the refilled activations are bitwise the ones the forward pass wrote; only the down-projection, whose
+// output xs[l + 1] is kept and not needed again, is skipped.
+int layer_fwd(dtx_trainer* t, int l, int phase, bool backward) {
+  const dtx_model_cfg& mc = t->mc;
+  const dtx_train_cfg& tc = t->tc;
+  const int d = mc.hidden, F = mc.ffn, M = t->cur_M, RP = t->RP, H = mc.n_heads, D = mc.head_dim;
+  const int Hkv = mc.n_kv_heads, W = t->W;
+  const int B = t->cur_B, S = t->cur_S;
+  const int32_t* seq_lens = t->use_seq_lens ? t->d_seq_lens : nullptr;
+  cudaStream_t s = t->stream;
+  const float att_scale = 1.0f / sqrtf(static_cast<float>(D));
+  const bool fused = use_fused(t);
+  const bool lora = !t->full;
+  const bool drop = lora && t->dropout;  // adapters laid out for per-target dropped inputs (KA = nt*d)
+  const float p_drop = backward ? tc.lora_dropout : 0.f;  // eval (model.eval()) runs the same path with p = 0
+  Layer& y = t->layers[l];
+  wait_weights(t, l);
+  CK(rmsnorm_fwd(t->xs[l], y.norm1, y.h1, y.rstd1, M, d, mc.rms_eps, s), 1);
+  const bf16* lora_in = y.h1;
+  if (drop) {  // peft: lora_A(lora_dropout(x)) with one nn.Dropout per wrapped module -> one dropped copy per target
+    CK(lora_dropout_fwd(y.h1, y.hd, M, d, t->nt, p_drop, dropout_key(t, l), s), 1);
+    lora_in = y.hd;
+  }
+  if (lora) {  // LoRA down-projection of all targets at once: t = lora_in * A_cat^T   [M, RP]
+    GemmArgs g;
+    g.A = lora_in; g.lda = t->KA; g.B = y.a_cat; g.ldb = t->KA; g.C = y.t; g.ldc = RP;
+    g.M = M; g.N = RP; g.K = t->KA; g.epilogue = EPI_BF16; g.block_n = 64;
+    CK(gemm_bf16(g, s), 1);
+  }
+  {  // qkv = h1 * Wqkv^T + t * B_ext^T : base projection and LoRA up-projection in one accumulator
+    BASEW(W_QKV, wqkv);
+    GemmArgs g;
+    g.A = y.h1; g.lda = d; g.B = wqkv; g.ldb = d;
+    if (lora) { g.A2 = y.t; g.lda2 = RP; g.B2 = y.b_ext; g.ldb2 = RP; g.K2 = RP; }
+    g.C = y.qkv; g.ldc = W; g.M = M; g.N = W; g.K = d; g.epilogue = EPI_BF16;
+    if (fused) {  // rotary embedding of q and k applied to the fp32 accumulator in the epilogue
+      g.epilogue = EPI_ROPE; g.rope_cs = t->rope_cs; g.rope_S = S; g.rope_cols = t->dq + t->dkv;
+      g.rope_pos = t->packed ? t->d_pos : nullptr;  // packed batch: a row's position is its offset inside its own sequence
+    }
+    CK(gemm_bf16(g, s), 1);
+  }
+  if (!fused && t->packed) return t->fail(DTX_ERR_STATE, "packed batches need the fused RoPE epilogue");
+  if (!fused) CK(rope_qk_inplace_table(y.qkv, t->rope_cs, B, S, H + Hkv, W, D, 0, s), 1);
+  {
+    AttnArgs a;
+    a.qkv = y.qkv; a.out = y.attn; a.lse = y.lse; a.B = B; a.S = S; a.H = H; a.Hkv = Hkv; a.scale = att_scale;
+    a.seq_lens = seq_lens; a.window = t->window;
+    if (t->packed) { a.row_start = t->d_row_start; a.total_rows = M; }
+    CK(attn_fwd(a, s), 1);
+  }
+  {  // x_mid = x + attn * Wo^T
+    BASEW(W_O, wo);
+    GemmArgs g;
+    g.A = y.attn; g.lda = d; g.B = wo; g.ldb = d; g.C = y.x_mid; g.ldc = d; g.R = t->xs[l]; g.ldr = d;
+    g.M = M; g.N = d; g.K = d; g.epilogue = EPI_BF16_ADD;
+    CK(gemm_bf16(g, s), 1);
+  }
+  CK(rmsnorm_fwd(y.x_mid, y.norm2, t->h2, y.rstd2, M, d, mc.rms_eps, s), 1);
+  {  // [gate | up] = h2 * Wgu^T
+    BASEW(W_GU, wgu);
+    GemmArgs g;
+    g.A = t->h2; g.lda = d; g.B = wgu; g.ldb = d; g.C = y.gu; g.ldc = 2 * F;
+    g.M = M; g.N = 2 * F; g.K = d; g.epilogue = EPI_BF16;
+    if (fused) {  // silu(gate) * up computed from the accumulator tile ([gate 128 | up 128] interleaved layout)
+      g.epilogue = EPI_SWIGLU_FWD; g.aux = t->act; g.ld_aux = F;
+    }
+    CK(gemm_bf16(g, s), 1);
+  }
+  if (!fused) CK(swiglu_fwd(y.gu, t->act, M, F, 1, s), 1);
+  if (phase == PH_FWD) {  // x_next = x_mid + act * Wdown^T
+    BASEW(W_DOWN, wdown);
+    GemmArgs g;
+    g.A = t->act; g.lda = F; g.B = wdown; g.ldb = F; g.C = t->xs[l + 1]; g.ldc = d; g.R = y.x_mid; g.ldr = d;
+    g.M = M; g.N = d; g.K = F; g.epilogue = EPI_BF16_ADD;
+    CK(gemm_bf16(g, s), 1);
+  }
+  return DTX_OK;
+}
+
 // forward (+ backward) of one micro-batch whose ids / labels (/ row lengths) are already in t->d_ids / t->d_labels (/ t->d_seq_lens).
 // The batch is [micro_batch, cur_S]: cur_S <= seq_len is this batch's own padded length (DataCollatorForSeq2Seq pads to the
 // longest row of the batch, cmd/tuning/train.py:282-286); every buffer was sized for seq_len.
@@ -606,13 +732,13 @@ int fwd_bwd(dtx_trainer* t, bool backward) {
   const int B = t->cur_B, S = t->cur_S;
   const int32_t* seq_lens = t->use_seq_lens ? t->d_seq_lens : nullptr;
   const int kb_tok = (M + 63) / 64;
-  const int split_b = std::min(t->split_b, pick_split((W + 127) / 128, kb_tok));
-  const int split_a = std::min(t->split_a, pick_split((t->KA + 127) / 128, kb_tok));
+  const int split_b = std::min(t->split_b, pick_split(gemm_num_sms(), (W + 127) / 128, kb_tok));
+  const int split_a = std::min(t->split_a, pick_split(gemm_num_sms(), (t->KA + 127) / 128, kb_tok));
   cudaStream_t s = t->stream;
   const float att_scale = 1.0f / sqrtf(static_cast<float>(D));
-  const bool fused = g_fused_epilogues && M > 128 && ((t->dq + t->dkv) % 256 == 0) && (W % 256 == 0);  // whole 256-column tiles
+  const bool fused = use_fused(t);
   const bool lora = !t->full;    // full-parameter SFT: no adapters, every weight gets a gradient
-  bool in_backward = false;      // which half of the step asks for a base weight (prefetch order of the NF4 expansion)
+  int phase = PH_FWD;            // which part of the step asks for a base weight (prefetch order of the NF4 expansion)
   const bool drop = lora && t->dropout;  // adapters laid out for per-target dropped inputs (KA = nt*d)
   const float p_drop = backward ? tc.lora_dropout : 0.f;  // eval (model.eval()) runs the same path with p = 0
   t->fwd_count += 1;
@@ -620,67 +746,8 @@ int fwd_bwd(dtx_trainer* t, bool backward) {
   wait_weights(t, L);  // globals (embedding, lm_head, final norm)
   CK(embedding_fwd(t->d_ids, t->embed, t->xs[0], M, d, V, s), 1);
   for (int l = 0; l < L; ++l) {
-    Layer& y = t->layers[l];
-    wait_weights(t, l);
-    CK(rmsnorm_fwd(t->xs[l], y.norm1, y.h1, y.rstd1, M, d, mc.rms_eps, s), 1);
-    const bf16* lora_in = y.h1;
-    if (drop) {  // peft: lora_A(lora_dropout(x)) with one nn.Dropout per wrapped module -> one dropped copy per target
-      CK(lora_dropout_fwd(y.h1, y.hd, M, d, t->nt, p_drop, dropout_key(t, l), s), 1);
-      lora_in = y.hd;
-    }
-    if (lora) {  // LoRA down-projection of all targets at once: t = lora_in * A_cat^T   [M, RP]
-      GemmArgs g;
-      g.A = lora_in; g.lda = t->KA; g.B = y.a_cat; g.ldb = t->KA; g.C = y.t; g.ldc = RP;
-      g.M = M; g.N = RP; g.K = t->KA; g.epilogue = EPI_BF16; g.block_n = 64;
-      CK(gemm_bf16(g, s), 1);
-    }
-    {  // qkv = h1 * Wqkv^T + t * B_ext^T : base projection and LoRA up-projection in one accumulator
-      BASEW(W_QKV, wqkv);
-      GemmArgs g;
-      g.A = y.h1; g.lda = d; g.B = wqkv; g.ldb = d;
-      if (lora) { g.A2 = y.t; g.lda2 = RP; g.B2 = y.b_ext; g.ldb2 = RP; g.K2 = RP; }
-      g.C = y.qkv; g.ldc = W; g.M = M; g.N = W; g.K = d; g.epilogue = EPI_BF16;
-      if (fused) {  // rotary embedding of q and k applied to the fp32 accumulator in the epilogue
-        g.epilogue = EPI_ROPE; g.rope_cs = t->rope_cs; g.rope_S = S; g.rope_cols = t->dq + t->dkv;
-        g.rope_pos = t->packed ? t->d_pos : nullptr;  // packed batch: a row's position is its offset inside its own sequence
-      }
-      CK(gemm_bf16(g, s), 1);
-    }
-    if (!fused && t->packed) return t->fail(DTX_ERR_STATE, "packed batches need the fused RoPE epilogue");
-    if (!fused) CK(rope_qk_inplace_table(y.qkv, t->rope_cs, B, S, H + Hkv, W, D, 0, s), 1);
-    {
-      AttnArgs a;
-      a.qkv = y.qkv; a.out = y.attn; a.lse = y.lse; a.B = B; a.S = S; a.H = H; a.Hkv = Hkv; a.scale = att_scale;
-      a.seq_lens = seq_lens; a.window = t->window;
-      if (t->packed) { a.row_start = t->d_row_start; a.total_rows = M; }
-      CK(attn_fwd(a, s), 1);
-    }
-    {  // x_mid = x + attn * Wo^T
-      BASEW(W_O, wo);
-      GemmArgs g;
-      g.A = y.attn; g.lda = d; g.B = wo; g.ldb = d; g.C = y.x_mid; g.ldc = d; g.R = t->xs[l]; g.ldr = d;
-      g.M = M; g.N = d; g.K = d; g.epilogue = EPI_BF16_ADD;
-      CK(gemm_bf16(g, s), 1);
-    }
-    CK(rmsnorm_fwd(y.x_mid, y.norm2, t->h2, y.rstd2, M, d, mc.rms_eps, s), 1);
-    {  // [gate | up] = h2 * Wgu^T
-      BASEW(W_GU, wgu);
-      GemmArgs g;
-      g.A = t->h2; g.lda = d; g.B = wgu; g.ldb = d; g.C = y.gu; g.ldc = 2 * F;
-      g.M = M; g.N = 2 * F; g.K = d; g.epilogue = EPI_BF16;
-      if (fused) {  // silu(gate) * up computed from the accumulator tile ([gate 128 | up 128] interleaved layout)
-        g.epilogue = EPI_SWIGLU_FWD; g.aux = t->act; g.ld_aux = F;
-      }
-      CK(gemm_bf16(g, s), 1);
-    }
-    if (!fused) CK(swiglu_fwd(y.gu, t->act, M, F, 1, s), 1);
-    {  // x_next = x_mid + act * Wdown^T
-      BASEW(W_DOWN, wdown);
-      GemmArgs g;
-      g.A = t->act; g.lda = F; g.B = wdown; g.ldb = F; g.C = t->xs[l + 1]; g.ldc = d; g.R = y.x_mid; g.ldr = d;
-      g.M = M; g.N = d; g.K = F; g.epilogue = EPI_BF16_ADD;
-      CK(gemm_bf16(g, s), 1);
-    }
+    int rc = layer_fwd(t, l, PH_FWD, backward);
+    if (rc) return rc;
   }
   // lm_head, CE and their backward only over the tokens that carry a label (shifted label >= 0): prompt tokens and padding
   // (27 % of the synthetic batch, far more on real instruction data) have zero loss and zero gradient.  The labelled rows
@@ -706,7 +773,7 @@ int fwd_bwd(dtx_trainer* t, bool backward) {
                            t->sub_ndiv), 1);
   CK(loss_reduce(t->row_loss, t->d_nvalid, t->d_loss, M, s, t->sub_ndiv, t->sub_accum ? 1 : 0), 1);
   if (!backward) return DTX_OK;
-  in_backward = true;
+  phase = PH_BWD;
 
   const int accumulate = (t->micro_idx > 0 || t->sub_accum) ? 1 : 0;
   // weight gradient of a Linear: dW[out, in] (+)= dY^T X - a token-contraction GEMM with both operands MN-major
@@ -732,6 +799,10 @@ int fwd_bwd(dtx_trainer* t, bool backward) {
   bf16* cur = t->dx_a;
   bf16* other = t->dx_b;
   for (int l = L - 1; l >= 0; --l) {
+    if (t->recompute == RECOMPUTE_LAYER && l < L - 1) {  // refill the shared saved set (the last layer's is still there)
+      int rc = layer_fwd(t, l, PH_RECOMPUTE, backward);
+      if (rc) return rc;
+    }
     Layer& y = t->layers[l];
     bf16* gl_w = t->full ? t->g_flat + static_cast<int64_t>(l) * t->layer_elems : nullptr;  // this layer's gradient block
     if (t->full) {  // dWdown = d x_out^T * act: act = silu(gate) * up is recomputed from the saved gate|up (one HBM-bound pass)
@@ -1204,6 +1275,78 @@ int target_index(const dtx_trainer* t, char which) {  // 'q','k','v' -> index am
   return -1;
 }
 
+// configuration checks of dtx_trainer_create and dtx_plan_device_bytes (host only; the message goes to g_error)
+int check_cfg(const dtx_model_cfg* mc, const dtx_train_cfg* tc) {
+  auto bad = [&](const char* m) {
+    g_error = m;
+    return DTX_ERR_INVALID;
+  };
+  if (mc->head_dim != 128) return bad("only head_dim 128 is implemented (Llama-2 / Mistral family)");
+  if (mc->n_kv_heads <= 0 || mc->n_heads % mc->n_kv_heads) return bad("n_heads must be a multiple of n_kv_heads");
+  if (mc->n_heads * mc->head_dim != mc->hidden) return bad("hidden != n_heads * head_dim");
+  if (mc->hidden % 64 || mc->ffn % 128 || mc->vocab % 8)
+    return bad("hidden must be a multiple of 64, ffn a multiple of 128 (GU-interleaved layout), vocab a multiple of 8");
+  if (tc->seq_len % 128 || tc->seq_len <= 0 || tc->micro_batch <= 0) return bad("seq_len must be a positive multiple of 128");
+  if (tc->seq_len > mc->max_seq) return bad("seq_len exceeds max_seq");
+  if (!tc->full_finetune && (tc->lora_r <= 0 || tc->lora_r % 8)) return bad("lora_r must be a positive multiple of 8");
+  if (tc->lora_dropout < 0.0f || tc->lora_dropout >= 1.0f) return bad("lora_dropout must be in [0, 1)");
+  if (tc->recompute < 0 || tc->recompute > RECOMPUTE_LAYER)
+    return bad("recompute must be 0 (automatic), 1 (keep all activations) or 2 (recompute per layer)");
+  if (!tc->full_finetune && ((tc->target_mask & ~(DTX_TARGET_Q | DTX_TARGET_K | DTX_TARGET_V)) || tc->target_mask == 0))
+    { g_error = "lora_target must be a non-empty subset of q_proj,k_proj,v_proj"; return DTX_ERR_UNSUPPORTED; }
+  return DTX_OK;
+}
+
+// shapes and adapter geometry derived from the configuration (host only)
+void setup_dims(dtx_trainer* t, const dtx_model_cfg* mc, const dtx_train_cfg* tc, int world) {
+  t->mc = *mc;
+  t->tc = *tc;
+  t->world = world;
+  t->M = tc->micro_batch * tc->seq_len;
+  t->dq = mc->n_heads * mc->head_dim;
+  t->dkv = mc->n_kv_heads * mc->head_dim;
+  t->W = t->dq + 2 * t->dkv;
+  t->full = tc->full_finetune != 0;
+  t->dropout = !t->full && tc->lora_dropout > 0.0f;
+  t->nt = 0;
+  t->per_layer = 0;
+  if (!t->full) {
+    const unsigned bits[3] = {DTX_TARGET_Q, DTX_TARGET_K, DTX_TARGET_V};
+    const char names[3] = {'q', 'k', 'v'};
+    const int row0[3] = {0, t->dq, t->dq + t->dkv};
+    const int dout[3] = {t->dq, t->dkv, t->dkv};
+    for (int i = 0; i < 3; ++i)
+      if (tc->target_mask & bits[i]) {
+        t->tg[t->nt].row0 = row0[i];
+        t->tg[t->nt].d_out = dout[i];
+        t->tg[t->nt].off = t->per_layer;
+        t->tg_name[t->nt] = names[i];
+        t->per_layer += static_cast<int64_t>(mc->hidden + dout[i]) * tc->lora_r;
+        ++t->nt;
+      }
+  }
+  t->RP = ((t->nt * tc->lora_r + 63) / 64) * 64;
+  t->KA = t->dropout ? t->nt * mc->hidden : mc->hidden;
+  t->n_train = static_cast<int64_t>(mc->n_layers) * t->per_layer;
+  t->cur_S = tc->seq_len;
+  t->cur_M = t->M;
+  // Mistral-style sliding window: only a different mask once the sequence is longer than the window
+  // (transformers 4.34.0 _make_sliding_window_causal_mask: triu(diagonal=-sliding_window), i.e. query i sees keys i - sw .. i)
+  t->window = (mc->sliding_window > 0 && tc->seq_len > mc->sliding_window + 1) ? mc->sliding_window : 0;
+}
+
+// device bytes create_buffers() allocates for this configuration and activation layout: the same function in a sizing run,
+// so that the plan cannot drift from the allocation (n_sms sizes the split-K partial buffers of the adapter gradients)
+int64_t planned_bytes(const dtx_model_cfg* mc, const dtx_train_cfg* tc, int world, int n_sms, int layout) {
+  dtx_trainer p;
+  setup_dims(&p, mc, tc, world);
+  p.n_sms = n_sms;
+  p.dry = true;
+  p.recompute = layout;
+  create_buffers(&p);
+  return static_cast<int64_t>(p.bytes_allocated);
+}
+
 }  // namespace
 
 // ==================================================================================================
@@ -1250,23 +1393,16 @@ int32_t dtx_trainer_create(const dtx_model_cfg* mc, const dtx_train_cfg* tc, int
     return DTX_ERR_INVALID;
   }
   *out = nullptr;
-  auto bad = [&](const char* m) {
-    g_error = m;
+  int rc = check_cfg(mc, tc);
+  if (rc) return rc;
+  if (world < 1 || rank < 0 || rank >= world) {
+    g_error = "bad rank/world";
     return DTX_ERR_INVALID;
-  };
-  if (mc->head_dim != 128) return bad("only head_dim 128 is implemented (Llama-2 / Mistral family)");
-  if (mc->n_kv_heads <= 0 || mc->n_heads % mc->n_kv_heads) return bad("n_heads must be a multiple of n_kv_heads");
-  if (mc->n_heads * mc->head_dim != mc->hidden) return bad("hidden != n_heads * head_dim");
-  if (mc->hidden % 64 || mc->ffn % 128 || mc->vocab % 8)
-    return bad("hidden must be a multiple of 64, ffn a multiple of 128 (GU-interleaved layout), vocab a multiple of 8");
-  if (tc->seq_len % 128 || tc->seq_len <= 0 || tc->micro_batch <= 0) return bad("seq_len must be a positive multiple of 128");
-  if (tc->seq_len > mc->max_seq) return bad("seq_len exceeds max_seq");
-  if (!tc->full_finetune && (tc->lora_r <= 0 || tc->lora_r % 8)) return bad("lora_r must be a positive multiple of 8");
-  if (tc->lora_dropout < 0.0f || tc->lora_dropout >= 1.0f) return bad("lora_dropout must be in [0, 1)");
-  if (!tc->full_finetune && ((tc->target_mask & ~(DTX_TARGET_Q | DTX_TARGET_K | DTX_TARGET_V)) || tc->target_mask == 0))
-    { g_error = "lora_target must be a non-empty subset of q_proj,k_proj,v_proj"; return DTX_ERR_UNSUPPORTED; }
-  if (world < 1 || rank < 0 || rank >= world) return bad("bad rank/world");
-  if (world > 1 && !nccl_unique_id) return bad("world > 1 needs an NCCL unique id");
+  }
+  if (world > 1 && !nccl_unique_id) {
+    g_error = "world > 1 needs an NCCL unique id";
+    return DTX_ERR_INVALID;
+  }
 
   cudaError_t e = cudaSetDevice(device);
   if (e != cudaSuccess) {
@@ -1280,43 +1416,40 @@ int32_t dtx_trainer_create(const dtx_model_cfg* mc, const dtx_train_cfg* tc, int
     return DTX_ERR_CUDA;
   }
   dtx_trainer* t = new dtx_trainer();
-  t->mc = *mc;
-  t->tc = *tc;
+  setup_dims(t, mc, tc, world);
   t->device = device;
   t->rank = rank;
-  t->world = world;
   if (prop.multiProcessorCount > 0) t->n_sms = prop.multiProcessorCount;
-  t->M = tc->micro_batch * tc->seq_len;
-  t->dq = mc->n_heads * mc->head_dim;
-  t->dkv = mc->n_kv_heads * mc->head_dim;
-  t->W = t->dq + 2 * t->dkv;
-  t->full = tc->full_finetune != 0;
-  t->dropout = !t->full && tc->lora_dropout > 0.0f;
-  t->nt = 0;
-  t->per_layer = 0;
-  if (!t->full) {
-    const unsigned bits[3] = {DTX_TARGET_Q, DTX_TARGET_K, DTX_TARGET_V};
-    const char names[3] = {'q', 'k', 'v'};
-    const int row0[3] = {0, t->dq, t->dq + t->dkv};
-    const int dout[3] = {t->dq, t->dkv, t->dkv};
-    for (int i = 0; i < 3; ++i)
-      if (tc->target_mask & bits[i]) {
-        t->tg[t->nt].row0 = row0[i];
-        t->tg[t->nt].d_out = dout[i];
-        t->tg[t->nt].off = t->per_layer;
-        t->tg_name[t->nt] = names[i];
-        t->per_layer += static_cast<int64_t>(mc->hidden + dout[i]) * tc->lora_r;
-        ++t->nt;
-      }
+  // Activation layout.  Automatic: keep every layer's activations when that fits in the free memory with kHeadroomBytes to
+  // spare (the bf16 base is resident at this point even for QLoRA, so this is the true peak), else recompute per layer.
+  t->recompute = tc->recompute ? tc->recompute : KEEP_ALL;
+  if (tc->recompute == 0) {
+    size_t free_b = 0, total_b = 0;
+    e = cudaMemGetInfo(&free_b, &total_b);
+    if (e != cudaSuccess) {
+      g_error = std::string("cudaMemGetInfo failed: ") + cudaGetErrorString(e);
+      delete t;
+      return DTX_ERR_CUDA;
+    }
+    const int64_t keep = planned_bytes(mc, tc, world, t->n_sms, KEEP_ALL);
+    const int64_t layer = planned_bytes(mc, tc, world, t->n_sms, RECOMPUTE_LAYER);
+    const int64_t avail = static_cast<int64_t>(free_b) - kHeadroomBytes;
+    if (keep <= avail) {
+      t->recompute = KEEP_ALL;
+    } else if (layer <= avail) {
+      t->recompute = RECOMPUTE_LAYER;
+    } else {
+      char buf[320];
+      snprintf(buf, sizeof(buf),
+               "device memory too small: keeping all activations needs %lld bytes, recomputing per layer %lld bytes, "
+               "%lld bytes are free (%lld kept in reserve)",
+               static_cast<long long>(keep), static_cast<long long>(layer), static_cast<long long>(free_b),
+               static_cast<long long>(kHeadroomBytes));
+      g_error = buf;
+      delete t;
+      return DTX_ERR_CUDA;
+    }
   }
-  t->RP = ((t->nt * tc->lora_r + 63) / 64) * 64;
-  t->KA = t->dropout ? t->nt * mc->hidden : mc->hidden;
-  t->n_train = static_cast<int64_t>(mc->n_layers) * t->per_layer;
-  t->cur_S = tc->seq_len;
-  t->cur_M = t->M;
-  // Mistral-style sliding window: only a different mask once the sequence is longer than the window
-  // (transformers 4.34.0 _make_sliding_window_causal_mask: triu(diagonal=-sliding_window), i.e. query i sees keys i - sw .. i)
-  t->window = (mc->sliding_window > 0 && tc->seq_len > mc->sliding_window + 1) ? mc->sliding_window : 0;
   cudaStreamCreateWithFlags(&t->stream, cudaStreamNonBlocking);
   cudaEventCreate(&t->ev0);
   cudaEventCreate(&t->ev1);
@@ -1331,7 +1464,7 @@ int32_t dtx_trainer_create(const dtx_model_cfg* mc, const dtx_train_cfg* tc, int
     for (auto& e : t->ev_ag) cudaEventCreateWithFlags(&e, cudaEventDisableTiming);
     t->ag_pending.assign(mc->n_layers + 1, 0);
   }
-  int rc = create_buffers(t);
+  rc = create_buffers(t);
   if (rc) {
     g_error = t->err;
     dtx_trainer_destroy(t);
@@ -1879,6 +2012,23 @@ int32_t dtx_export_weight(dtx_trainer* t, const char* name, void* host_out, int6
 }
 
 int64_t dtx_num_trainable(const dtx_trainer* t) { return t ? t->n_train : 0; }
+int32_t dtx_recompute(const dtx_trainer* t) { return t ? t->recompute : DTX_ERR_INVALID; }
+int64_t dtx_device_bytes(const dtx_trainer* t) { return t ? static_cast<int64_t>(t->bytes_allocated) : 0; }
+
+int32_t dtx_plan_device_bytes(const dtx_model_cfg* mc, const dtx_train_cfg* tc, int32_t world, int32_t layout, int64_t* bytes_out) {
+  if (!mc || !tc || !bytes_out || world < 1) {
+    g_error = "plan_device_bytes: null argument or world < 1";
+    return DTX_ERR_INVALID;
+  }
+  if (layout != KEEP_ALL && layout != RECOMPUTE_LAYER) {
+    g_error = "plan_device_bytes: layout must be 1 (keep all activations) or 2 (recompute per layer)";
+    return DTX_ERR_INVALID;
+  }
+  const int rc = check_cfg(mc, tc);
+  if (rc) return rc;
+  *bytes_out = planned_bytes(mc, tc, world, 132, layout);  // split-K buffers sized for the 132 SMs of an H100 SXM
+  return DTX_OK;
+}
 int64_t dtx_launch_count(const dtx_trainer* t) { return t ? t->launches : 0; }
 float dtx_last_step_ms(const dtx_trainer* t) { return t ? t->last_ms : 0.f; }
 int32_t dtx_last_step_groups(const dtx_trainer* t) { return t ? t->last_groups : 0; }

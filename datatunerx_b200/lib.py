@@ -22,6 +22,8 @@ SCHED = {"linear": 0, "cosine": 1, "constant": 2, "constant_with_warmup": 3}
 TARGET_BITS = {"q_proj": 1, "k_proj": 2, "v_proj": 4}
 EPI_BF16, EPI_F32, EPI_BF16_ADD, EPI_ROPE, EPI_SWIGLU_FWD, EPI_SWIGLU_BWD = 0, 1, 2, 3, 4, 5
 STEP_FORCE = 1
+# activation layouts (dtx_train_cfg.recompute): automatic, every layer keeps its activations, one shared set recomputed per layer
+RECOMPUTE = {"auto": 0, "keep": 1, "layer": 2}
 
 
 class DtxError(RuntimeError):
@@ -42,7 +44,7 @@ class TrainCfg(C.Structure):
                 ("beta2", C.c_float), ("eps", C.c_float), ("max_grad_norm", C.c_float), ("sched", C.c_int32),
                 ("warmup_steps", C.c_int32), ("total_steps", C.c_int32), ("grad_accum", C.c_int32),
                 ("micro_batch", C.c_int32), ("seq_len", C.c_int32), ("seed", C.c_uint64), ("full_finetune", C.c_int32),
-                ("reserved", C.c_int32)]
+                ("recompute", C.c_int32)]
 
 
 # every symbol include/dtxtune.h declares (tests/test_abi.py checks the .so exports all of them)
@@ -50,6 +52,7 @@ ABI_SYMBOLS = [
     "dtx_abi_version", "dtx_last_global_error", "dtx_last_error", "dtx_trainer_create", "dtx_trainer_destroy",
     "dtx_get_nccl_unique_id", "dtx_load_tensor", "dtx_init_random_weights", "dtx_init_lora", "dtx_quantize_base", "dtx_step",
     "dtx_step_device", "dtx_eval_loss", "dtx_allreduce_host", "dtx_export_adapter", "dtx_export_adapter_grad", "dtx_export_weight", "dtx_num_trainable", "dtx_launch_count",
+    "dtx_recompute", "dtx_device_bytes", "dtx_plan_device_bytes",
     "dtx_base_weight_bytes", "dtx_last_step_ms", "dtx_last_step_timings", "dtx_last_step_groups", "dtx_plan_length_groups", "dtx_plan_packed_rows", "dtx_lr_lambda", "dtx_set_option", "dtx_gemm_bf16",
     "dtx_gemm_fused", "dtx_embedding_fwd", "dtx_rmsnorm_fwd", "dtx_rmsnorm_bwd",
     "dtx_rope_table", "dtx_rope_qk", "dtx_swiglu_fwd", "dtx_swiglu_bwd", "dtx_lora_dropout_fwd", "dtx_lora_dropout_bwd_add",
@@ -102,6 +105,10 @@ def load() -> C.CDLL:
     lib.dtx_export_weight.argtypes = [vp, C.c_char_p, vp, i64, i32]
     lib.dtx_num_trainable.argtypes = [vp]
     lib.dtx_num_trainable.restype = i64
+    lib.dtx_recompute.argtypes = [vp]
+    lib.dtx_device_bytes.argtypes = [vp]
+    lib.dtx_device_bytes.restype = i64
+    lib.dtx_plan_device_bytes.argtypes = [C.POINTER(ModelCfg), C.POINTER(TrainCfg), i32, i32, C.POINTER(i64)]
     lib.dtx_launch_count.argtypes = [vp]
     lib.dtx_launch_count.restype = i64
     lib.dtx_last_step_ms.argtypes = [vp]
@@ -169,6 +176,15 @@ def plan_length_groups(model: "ModelConfig", seq_lens, seq_len_batch: int, n_sms
     return [([int(r) for r in order[start[g]:start[g + 1]]], int(glen[g])) for g in range(n)]
 
 
+def plan_device_bytes(model: "ModelConfig", train: "TrainConfig", world: int = 1, layout="keep") -> int:
+    """Bytes of device memory a trainer for this configuration allocates per rank with activation layout "keep" or "layer"
+    (host arithmetic inside the library, no GPU needed)."""
+    code = RECOMPUTE[layout] if isinstance(layout, str) else int(layout)
+    mc, tc, out = model.to_c(), train.to_c(), C.c_int64()
+    check(load().dtx_plan_device_bytes(C.byref(mc), C.byref(tc), world, code, C.byref(out)))
+    return int(out.value)
+
+
 def lr_lambda(sched: str, step: int, warmup: int, total: int) -> float:
     """HF get_scheduler multiplier — host arithmetic inside the library, usable without a GPU."""
     return float(load().dtx_lr_lambda(SCHED[sched], step, warmup, total))
@@ -217,8 +233,11 @@ class TrainConfig:
     grad_accum: int = 1
     seed: int = 42
     full_finetune: bool = False         # every weight trains, no adapters (BASELINE.json configs[3]; beyond the reference)
+    recompute: str = "auto"             # activation layout: "auto", "keep" (every layer keeps its own) or "layer" (recompute per layer)
 
     def to_c(self) -> TrainCfg:
+        if self.recompute not in RECOMPUTE:
+            raise DtxError(-1, f"recompute {self.recompute!r}: expected one of {', '.join(RECOMPUTE)}")
         mask = 0
         for t in self.lora_target:
             if t not in TARGET_BITS:
@@ -226,7 +245,8 @@ class TrainConfig:
             mask |= TARGET_BITS[t]
         return TrainCfg(self.lora_r, self.lora_alpha, self.lora_dropout, mask, self.lr, self.weight_decay, self.beta1,
                         self.beta2, self.eps, self.max_grad_norm, SCHED[self.sched], self.warmup_steps, self.total_steps,
-                        self.grad_accum, self.micro_batch, self.seq_len, self.seed, 1 if self.full_finetune else 0, 0)
+                        self.grad_accum, self.micro_batch, self.seq_len, self.seed, 1 if self.full_finetune else 0,
+                        RECOMPUTE[self.recompute])
 
 
 _NP_DTYPES = {np.dtype(np.float32): DTX_F32, np.dtype(np.float16): DTX_F16}
@@ -390,6 +410,17 @@ class Trainer:
     @property
     def num_trainable(self) -> int:
         return int(self.lib.dtx_num_trainable(self._h))
+
+    @property
+    def recompute(self) -> str:
+        """Activation layout in use: "keep" or "layer" (what "auto" chose)."""
+        code = int(self.lib.dtx_recompute(self._h))
+        return {v: k for k, v in RECOMPUTE.items()}[code]
+
+    @property
+    def device_bytes(self) -> int:
+        """Bytes of device memory the trainer holds now."""
+        return int(self.lib.dtx_device_bytes(self._h))
 
     @property
     def launch_count(self) -> int:

@@ -105,6 +105,10 @@ def run_rank(a: TrainArgs, rank: int, world: int, nccl_id: Optional[bytes], toke
         L.set_option(name.strip(), int(value))  # an unknown name raises (DTX_ERR_INVALID)
     device = int(os.environ.get("DTX_DEVICE", rank))
     tr = L.Trainer(mc, tc, device=device, rank=rank, world=world, nccl_id=nccl_id)
+    if rank == 0:  # --gradient_checkpointing is ignored (the reference hard-codes it): the library picks what fits the device
+        keep, layer = (L.plan_device_bytes(mc, tc, world, k) for k in ("keep", "layer"))
+        print(f"[dtx] activations: {'recompute per layer' if tr.recompute == 'layer' else 'keep all'} "
+              f"(planned device bytes per rank: keep all {keep / 1e9:.1f} GB, recompute per layer {layer / 1e9:.1f} GB)", flush=True)
     if os.environ.get("DTX_RANDOM_INIT"):  # benchmarking / scheduling harnesses: config.json only, N(0, 0.02) weights on the device
         tr.init_random_weights(int(os.environ["DTX_RANDOM_INIT"]))
     else:

@@ -76,7 +76,15 @@ typedef struct {
    * sharded over the data-parallel ranks (ZeRO-1), gradients reduce-scattered per layer while the backward pass runs,
    * updated weights all-gathered; AdamW weight decay skips the RMSNorm weights (HF Trainer.get_decay_parameter_names). */
   int32_t full_finetune;
-  int32_t reserved;
+  /* Activations the backward pass needs (per layer h1, the LoRA t and dropped inputs, qkv, attn, lse, rstd1, x_mid, rstd2, gu):
+   *   1 = keep all: every layer keeps its own copy (fastest; 93 KB per token and layer for Llama-2-7B LoRA).
+   *   2 = recompute per layer (HF gradient checkpointing): one copy shared by all layers; the backward pass re-runs each
+   *       layer's forward (q|k|v, o, gate|up GEMMs and attention; not the down-projection) from the kept residual stream
+   *       before its backward.  Same kernels on the same inputs: results are bitwise identical to 1.
+   *   0 = automatic: 1 when its bytes (dtx_plan_device_bytes) plus 1 GiB fit in the free device memory at dtx_trainer_create,
+   *       else 2 when that fits, else dtx_trainer_create fails with DTX_ERR_CUDA and both sizes in the message.
+   * Other values: DTX_ERR_INVALID.  The reference always trains with gradient_checkpointing=True (train.py:214,252). */
+  int32_t recompute;
 } dtx_train_cfg;
 
 typedef struct dtx_trainer dtx_trainer;
@@ -152,6 +160,14 @@ DTX_API int32_t dtx_export_adapter_grad(dtx_trainer* t, const char* hf_name, voi
  * in the HF layout - what trainer.save_model writes for a full fine-tune. */
 DTX_API int32_t dtx_export_weight(dtx_trainer* t, const char* hf_name, void* host_out_bf16, int64_t nbytes, int32_t grad);
 DTX_API int64_t dtx_num_trainable(const dtx_trainer* t);
+/* activation layout in use: 1 = keep all, 2 = recompute per layer (dtx_train_cfg.recompute) */
+DTX_API int32_t dtx_recompute(const dtx_trainer* t);
+/* bytes of device memory the trainer holds now (drops after dtx_quantize_base) */
+DTX_API int64_t dtx_device_bytes(const dtx_trainer* t);
+/* Bytes dtx_trainer_create allocates for this configuration, `world` ranks and activation layout (1 or 2; host arithmetic, no
+ * device).  The small split-K partial buffers of the adapter gradients are sized for the 132 SMs of an H100 SXM. */
+DTX_API int32_t dtx_plan_device_bytes(const dtx_model_cfg* model, const dtx_train_cfg* train, int32_t world, int32_t layout,
+                                      int64_t* bytes_out);
 /* kernels launched by this trainer since creation (bench.py's gpu_launches) */
 DTX_API int64_t dtx_launch_count(const dtx_trainer* t);
 /* device time of the most recent dtx_step in ms (CUDA events on the trainer's stream) */
