@@ -139,6 +139,12 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* s
                "r"(smem_u32(src)), "r"(x), "r"(y)
                : "memory");
 }
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, const void* src, int x, int y, int z) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
+                   reinterpret_cast<uint64_t>(m)),
+               "r"(smem_u32(src)), "r"(x), "r"(y), "r"(z)
+               : "memory");
+}
 // barrier among `nthreads` threads (a multiple of 32) of the CTA on hardware barrier `id` (1..15; 0 is __syncthreads)
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
@@ -267,6 +273,17 @@ __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefe
 // after which the compiler only knows a generic pointer and would emit slower generic LD/ST
 __device__ __forceinline__ void sts128(uint32_t saddr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+}
+__device__ __forceinline__ void sts32(uint32_t saddr, uint32_t a) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(saddr), "r"(a) : "memory");
+}
+__device__ __forceinline__ void sts64f(uint32_t saddr, float a, float b) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(saddr), "f"(a), "f"(b) : "memory");
+}
+__device__ __forceinline__ uint32_t lds32(uint32_t saddr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(saddr) : "memory");
+  return v;
 }
 __device__ __forceinline__ float4 lds128f(uint32_t saddr) {
   float4 v;

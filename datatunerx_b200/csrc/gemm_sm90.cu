@@ -8,8 +8,13 @@
 //                                  shared-memory ring; the warpgroup hands its registers to the consumers (setmaxnreg)
 //   warpgroups 1, 2 consumers    : each owns 64 rows of the tile, issues wgmma.mma_async (64 x BN x 16 per instruction) on the
 //                                  ring slots and keeps its 64 x BN fp32 accumulator in registers; the epilogue (convert /
-//                                  +residual / rotary / SwiGLU) runs on those registers while the producer already fills the
-//                                  ring for the next tile
+//                                  +residual / rotary / SwiGLU) runs on those registers
+// Epilogue: each consumer warpgroup owns a 16 KB staging half (two 64-row x 128-byte boxes, 128B swizzle, the TMA layout) and
+// emits its slice of the tile in passes of two boxes: registers -> st.shared -> cp.async.bulk.tensor store. It then goes
+// straight on to the next tile's main loop while the stores drain; before it writes the staging half again it waits until the
+// previous bulk stores have read it. Epilogue inputs (the residual of EPI_BF16_ADD, gu of EPI_SWIGLU_BWD) are TMA-loaded into
+// the same staging boxes and updated in place; the first pass's input is requested before the last k-block's wgmma retires.
+// Rows >= M and columns beyond the output are clipped by the tensor maps' bounds.
 // The contraction may be extended by a second (A2,B2) segment: that is how the rank-r LoRA update is
 // accumulated into the same accumulator as the frozen base weight (one extra k-block, no extra pass).
 #include "common.cuh"
@@ -43,6 +48,7 @@ struct GemmKParams {
   int rope_S, rope_cols, rope_inverse;
   const int32_t* rope_pos;  // optional per-row position (packed ragged batches); null: row % rope_S
   const int32_t* m_eff;  // device-side row count; 256-row blocks that start at or beyond it are skipped
+  int c_cols, x_cols;    // inner extents of the tmC / tmX tensor maps: output boxes at or beyond them are not issued
 };
 
 template <int BN>
@@ -50,57 +56,30 @@ struct GemmCfg {
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = (BN == 256) ? 4 : ((BN == 128) ? 6 : 8);  // 192 KB of the 227 KB a block may have
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int STAGES = (BN == 256) ? 4 : ((BN == 128) ? 6 : 8);  // 192 KB ring
+  static constexpr int RING_BYTES = STAGES * STAGE_BYTES;
+  static constexpr int BOX_BYTES = 64 * 128;             // one staging box: 64 rows x 128 bytes (64 bf16 or 32 fp32 columns)
+  static constexpr int STG_BYTES = 2 * 2 * BOX_BYTES;    // two boxes per consumer warpgroup
+  // 230 656 of the 232 448 bytes a block may opt into
+  static constexpr int SMEM_BYTES = RING_BYTES + STG_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 };
-
-// store two neighbouring accumulator columns (col even) of one row with the plain epilogues
-template <int EPI>
-__device__ __forceinline__ void store_pair(const GemmKParams& p, int row, int col, int split, float v0, float v1) {
-  if (col >= p.N) return;
-  const bool both = col + 1 < p.N;
-  if (EPI == EPI_F32) {
-    float* c = reinterpret_cast<float*>(p.C) + static_cast<long long>(split) * p.M * p.ldc + static_cast<long long>(row) * p.ldc + col;
-    if (both && ((reinterpret_cast<uintptr_t>(c) & 7) == 0)) {
-      *reinterpret_cast<float2*>(c) = make_float2(v0, v1);
-    } else {
-      c[0] = v0;
-      if (both) c[1] = v1;
-    }
-  } else {
-    bf16* c = reinterpret_cast<bf16*>(p.C) + static_cast<long long>(row) * p.ldc + col;
-    if (EPI == EPI_BF16_ADD) {
-      const bf16* r = p.R + static_cast<long long>(row) * p.ldr + col;
-      if (both && ((reinterpret_cast<uintptr_t>(r) & 3) == 0)) {
-        const float2 rr = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(r));
-        v0 += rr.x;
-        v1 += rr.y;
-      } else {
-        v0 += __bfloat162float(r[0]);
-        if (both) v1 += __bfloat162float(r[1]);
-      }
-    }
-    if (both && ((reinterpret_cast<uintptr_t>(c) & 3) == 0)) {
-      *reinterpret_cast<uint32_t*>(c) = pack_bf16x2(v0, v1);
-    } else {
-      c[0] = __float2bfloat16_rn(v0);
-      if (both) c[1] = __float2bfloat16_rn(v1);
-    }
-  }
-}
 
 __device__ __forceinline__ float round_bf16(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
 
+// tmC: the output C (fp32: 3-D [split][M][N] with box {32, 64, 1}; bf16: 2-D with box {64, 64});
+// tmX: the second operand of the epilogue (R of EPI_BF16_ADD, act of EPI_SWIGLU_FWD, gu of EPI_SWIGLU_BWD), bf16 box {64, 64}
 template <int BN, bool A_MN, bool B_MN, int EPI>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-            const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2, const GemmKParams p) {
+            const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
+            const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmX, const GemmKParams p) {
   using Cfg = GemmCfg<BN>;
   static_assert(EPI < EPI_ROPE || BN == 256, "the fused epilogues pair columns 64 / 128 apart inside one 256-column tile");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::RING_BYTES + Cfg::STG_BYTES);
   uint64_t* empty_bar = full_bar + Cfg::STAGES;
+  uint64_t* x_bar = empty_bar + Cfg::STAGES;  // one per consumer warpgroup: its epilogue-input tiles have landed
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -111,10 +90,14 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     tma_prefetch_desc(&tmB);
     tma_prefetch_desc(&tmA2);
     tma_prefetch_desc(&tmB2);
+    tma_prefetch_desc(&tmC);
+    tma_prefetch_desc(&tmX);
     for (int i = 0; i < Cfg::STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 8);  // lane 0 of each of the eight consumer warps
     }
+    mbar_init(&x_bar[0], 1);
+    mbar_init(&x_bar[1], 1);
     fence_barrier_init();
   }
   __syncthreads();
@@ -185,14 +168,62 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     const int cw = wg - 1;                 // rows 64 * cw .. + 63 of the tile
     const int wq = warp & 3;               // warp inside the warpgroup
     const int rq = lane >> 2, cq = (lane & 3) * 2;
+    const bool issuer = (threadIdx.x & 127) == 0;  // issues this warpgroup's epilogue bulk copies and waits for them
+    uint8_t* stg = smem + Cfg::RING_BYTES + cw * 2 * Cfg::BOX_BYTES;
+    const uint32_t stg_u = smem_u32(stg);
+    uint32_t x_phase = 0;
     int stage = 0;
     uint32_t phase = 0;
     float acc[BN / 2];
+
+    // staging address of this thread's element pair in row wq * 16 + rq + 8 * hr of box `box`: 16-byte chunk `ch`, byte `b`
+    auto sa = [&](int hr, int box, int ch, int b) -> uint32_t {
+      return stg_u + box * Cfg::BOX_BYTES + sw128_offset(wq * 16 + rq + 8 * hr, ch) + b;
+    };
+    // the staging half is written only once the bulk stores of the previous pass have read it
+    auto pass_begin = [&]() {
+      if (issuer) tma_store_wait_read0();
+      named_bar_sync(1 + cw, 128);
+    };
+    // TMA-load the tmX boxes at columns x0 + b * dx (b < nbox), rows y .. y + 63, into the staging half
+    auto x_load = [&](int x0, int dx, int nbox, int y) {
+      if (issuer) {
+        tma_store_wait_read0();
+        uint32_t bytes = 0;
+        for (int b = 0; b < nbox; ++b)
+          if (y < p.M && x0 + b * dx < p.x_cols) bytes += Cfg::BOX_BYTES;
+        mbar_arrive_expect_tx(&x_bar[cw], bytes);
+        for (int b = 0; b < nbox; ++b)
+          if (y < p.M && x0 + b * dx < p.x_cols) tma_load_2d(stg + b * Cfg::BOX_BYTES, &tmX, &x_bar[cw], x0 + b * dx, y);
+      }
+    };
+    auto x_wait = [&]() {
+      mbar_wait(&x_bar[cw], x_phase);
+      x_phase ^= 1u;
+    };
+    // hand the pass to the async proxy and store its boxes to columns x0 + b * dx of `m` (split z of an fp32 output)
+    auto pass_store = [&](const CUtensorMap* m, int cols, int x0, int dx, int nbox, int y, int z) {
+      fence_proxy_async_smem();
+      named_bar_sync(1 + cw, 128);
+      if (issuer) {
+        for (int b = 0; b < nbox; ++b) {
+          if (y >= p.M || x0 + b * dx >= cols) continue;
+          if (EPI == EPI_F32) {
+            tma_store_3d(m, stg + b * Cfg::BOX_BYTES, x0 + b * dx, y, z);
+          } else {
+            tma_store_2d(m, stg + b * Cfg::BOX_BYTES, x0 + b * dx, y);
+          }
+        }
+        tma_store_commit();
+      }
+    };
+
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       int m_blk, n_blk, split, kb_begin, kb_end;
       decode(tile, m_blk, n_blk, split, kb_begin, kb_end);
       if (dead(m_blk)) continue;
       const int m0 = m_blk * BM, n0 = n_blk * BN;
+      const int y0 = m0 + cw * 64;  // first row of this warpgroup's slice
       int prev = -1;
       for (int kb = kb_begin; kb < kb_end; ++kb) {
         mbar_wait(&full_bar[stage], phase);
@@ -213,77 +244,149 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         prev = stage;
         if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1u; }
       }
+      // the first pass's epilogue input is requested while the last k-block's MMAs run
+      if (EPI == EPI_BF16_ADD) x_load(n0, 64, BN >= 128 ? 2 : 1, y0);
+      if (EPI == EPI_SWIGLU_BWD) x_load(2 * n0, 128, 2, y0);
       wgmma_wait<0>();
       wgmma_touch(acc);
       if (lane == 0) mbar_arrive(&empty_bar[prev]);
 
-      // ------------------------------ epilogue on the accumulator fragment ------------------------------
+      // ------------------------------ epilogue: accumulator fragment -> staging boxes -> bulk stores ------------------------------
+      if (EPI == EPI_BF16 || EPI == EPI_BF16_ADD) {
+        constexpr int NB = BN >= 128 ? 2 : 1;  // 64-column boxes per pass
 #pragma unroll
-      for (int hr = 0; hr < 2; ++hr) {
-        const int row = m0 + cw * 64 + wq * 16 + rq + hr * 8;
-        if (row >= p.M) continue;
-        if (EPI == EPI_ROPE) {
-          // two heads per tile (columns 0-127 / 128-255); rotary pairs column i with i + 64 of a head
-          const bool rot = n0 < p.rope_cols;
-          const float2* cs = p.rope_cs + static_cast<long long>(p.rope_pos ? __ldg(p.rope_pos + row) : row % p.rope_S) * 64;
+        for (int ps = 0; ps < BN / (64 * NB); ++ps) {
+          if (EPI == EPI_BF16_ADD) {
+            if (ps > 0) x_load(n0 + 128 * ps, 64, NB, y0);
+            x_wait();
+          } else {
+            pass_begin();
+          }
 #pragma unroll
-          for (int hh = 0; hh < 2; ++hh) {
+          for (int jj = 0; jj < 8 * NB; ++jj) {
+            const int j = ps * 8 * NB + jj;
 #pragma unroll
-            for (int jj = 0; jj < 8; ++jj) {
-              const int jl = hh * 16 + jj, jh = jl + 8;
+            for (int hr = 0; hr < 2; ++hr) {
+              const uint32_t a = sa(hr, jj >> 3, jj & 7, cq * 2);
+              float v0 = acc[4 * j + 2 * hr], v1 = acc[4 * j + 2 * hr + 1];
+              if (EPI == EPI_BF16_ADD) {  // the residual tile sits where the output goes
+                const float2 rr = unpack_bf16x2(lds32(a));
+                v0 += rr.x;
+                v1 += rr.y;
+              }
+              sts32(a, pack_bf16x2(v0, v1));
+            }
+          }
+          pass_store(&tmC, p.c_cols, n0 + 128 * ps, 64, NB, y0, 0);
+        }
+      } else if (EPI == EPI_F32) {
+        // 64 columns per pass: two boxes of 32 fp32 columns
+#pragma unroll
+        for (int ps = 0; ps < BN / 64; ++ps) {
+          pass_begin();
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const int j = ps * 8 + jj;
+#pragma unroll
+            for (int hr = 0; hr < 2; ++hr)
+              sts64f(sa(hr, jj >> 2, (jj & 3) * 2 + (cq >> 2), (cq & 3) * 4), acc[4 * j + 2 * hr], acc[4 * j + 2 * hr + 1]);
+          }
+          pass_store(&tmC, p.c_cols, n0 + 64 * ps, 32, 2, y0, split);
+        }
+      } else if (EPI == EPI_ROPE) {
+        // two heads per tile (columns 0-127 / 128-255), one per pass; rotary pairs column i with i + 64 of a head
+        const bool rot = n0 < p.rope_cols;
+        const float2* cs[2];
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          const int row = y0 + wq * 16 + rq + 8 * hr;
+          const int pos = row >= p.M ? 0 : (p.rope_pos ? __ldg(p.rope_pos + row) : row % p.rope_S);
+          cs[hr] = p.rope_cs + static_cast<long long>(pos) * 64;
+        }
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          pass_begin();
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const int jl = hh * 16 + jj, jh = jl + 8;
+#pragma unroll
+            for (int hr = 0; hr < 2; ++hr) {
               float lo[2] = {acc[4 * jl + 2 * hr], acc[4 * jl + 2 * hr + 1]}, hi[2] = {acc[4 * jh + 2 * hr], acc[4 * jh + 2 * hr + 1]};
               if (rot) {
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
-                  const float2 t = __ldg(cs + jj * 8 + cq + e);
+                  const float2 t = __ldg(cs[hr] + jj * 8 + cq + e);
                   const float sn = p.rope_inverse ? -t.y : t.y;
                   const float x0 = lo[e], x1 = hi[e];
                   lo[e] = x0 * t.x - x1 * sn;
                   hi[e] = x1 * t.x + x0 * sn;
                 }
               }
-              store_pair<EPI_BF16>(p, row, n0 + jl * 8 + cq, 0, lo[0], lo[1]);
-              store_pair<EPI_BF16>(p, row, n0 + jh * 8 + cq, 0, hi[0], hi[1]);
+              sts32(sa(hr, 0, jj, cq * 2), pack_bf16x2(lo[0], lo[1]));
+              sts32(sa(hr, 1, jj, cq * 2), pack_bf16x2(hi[0], hi[1]));
             }
           }
-        } else if (EPI == EPI_SWIGLU_FWD) {
-          // tile = [gate 128 | up 128] of the same 128 features
-          bf16* arow = reinterpret_cast<bf16*>(p.aux) + static_cast<long long>(row) * p.ld_aux + (n0 >> 1);
+          pass_store(&tmC, p.c_cols, n0 + 128 * hh, 64, 2, y0, 0);
+        }
+      } else if (EPI == EPI_SWIGLU_FWD) {
+        // tile = [gate 128 | up 128] of the same 128 features: pass 0 stores gate and pass 1 up to C, pass 2 the activation to aux
+#pragma unroll
+        for (int ps = 0; ps < 3; ++ps) {
+          pass_begin();
 #pragma unroll
           for (int j = 0; j < 16; ++j) {
-            const float g0 = acc[4 * j + 2 * hr], g1 = acc[4 * j + 2 * hr + 1];
-            const float u0 = acc[4 * (j + 16) + 2 * hr], u1 = acc[4 * (j + 16) + 2 * hr + 1];
-            store_pair<EPI_BF16>(p, row, n0 + j * 8 + cq, 0, g0, g1);
-            store_pair<EPI_BF16>(p, row, n0 + 128 + j * 8 + cq, 0, u0, u1);
-            // like the unfused path, gate/up are rounded to bf16 before the activation (fast reciprocal: ~1 ulp apart)
-            const float gg0 = round_bf16(g0), gg1 = round_bf16(g1), uu0 = round_bf16(u0), uu1 = round_bf16(u1);
-            *reinterpret_cast<uint32_t*>(arow + j * 8 + cq) =
-                pack_bf16x2(gg0 * __fdividef(1.f, 1.f + __expf(-gg0)) * uu0, gg1 * __fdividef(1.f, 1.f + __expf(-gg1)) * uu1);
-          }
-        } else if (EPI == EPI_SWIGLU_BWD) {
-          // acc = d(act) for features n0 + 8j + cq + e; gate/up of feature f live at (f/128)*256 + f%128 (+128) of gu / d(gu)
-          const bf16* grow = reinterpret_cast<const bf16*>(p.aux) + static_cast<long long>(row) * p.ld_aux;
-          bf16* crow = reinterpret_cast<bf16*>(p.C) + static_cast<long long>(row) * p.ldc;
 #pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const int f = n0 + j * 8 + cq;
-            if (f >= p.N) break;
-            const long long gc = static_cast<long long>(f >> 7) * 256 + (f & 127);
-            const float2 g2 = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(grow + gc));
-            const float2 u2 = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(grow + gc + 128));
-            // d(act) is rounded to bf16 first, exactly like the unfused path that stores it
-            const float d0 = round_bf16(acc[4 * j + 2 * hr]), d1 = round_bf16(acc[4 * j + 2 * hr + 1]);
-            const float s0 = __fdividef(1.f, 1.f + __expf(-g2.x)), s1 = __fdividef(1.f, 1.f + __expf(-g2.y));
-            const float si0 = g2.x * s0, si1 = g2.y * s1;
-            *reinterpret_cast<uint32_t*>(crow + gc) = pack_bf16x2(d0 * u2.x * (s0 + si0 * (1.f - s0)), d1 * u2.y * (s1 + si1 * (1.f - s1)));
-            *reinterpret_cast<uint32_t*>(crow + gc + 128) = pack_bf16x2(d0 * si0, d1 * si1);
+            for (int hr = 0; hr < 2; ++hr) {
+              const float g0 = acc[4 * j + 2 * hr], g1 = acc[4 * j + 2 * hr + 1];
+              const float u0 = acc[4 * (j + 16) + 2 * hr], u1 = acc[4 * (j + 16) + 2 * hr + 1];
+              uint32_t v;
+              if (ps == 0) {
+                v = pack_bf16x2(g0, g1);
+              } else if (ps == 1) {
+                v = pack_bf16x2(u0, u1);
+              } else {
+                // like the unfused path, gate/up are rounded to bf16 before the activation (fast reciprocal: ~1 ulp apart)
+                const float gg0 = round_bf16(g0), gg1 = round_bf16(g1), uu0 = round_bf16(u0), uu1 = round_bf16(u1);
+                v = pack_bf16x2(gg0 * __fdividef(1.f, 1.f + __expf(-gg0)) * uu0, gg1 * __fdividef(1.f, 1.f + __expf(-gg1)) * uu1);
+              }
+              sts32(sa(hr, j >> 3, j & 7, cq * 2), v);
+            }
           }
-        } else {
+          if (ps < 2) {
+            pass_store(&tmC, p.c_cols, n0 + 128 * ps, 64, 2, y0, 0);
+          } else {
+            pass_store(&tmX, p.x_cols, n0 >> 1, 64, 2, y0, 0);
+          }
+        }
+      } else {
+        // EPI_SWIGLU_BWD: acc = d(act) for features n0 + 8j + cq + e; gate/up of feature f live at (f/128)*256 + f%128 (+128) of
+        // gu / d(gu). Pass q covers features n0 + 64q .. + 63: their gate and up columns are one box each, rewritten in place.
 #pragma unroll
-          for (int j = 0; j < BN / 8; ++j) store_pair<EPI>(p, row, n0 + j * 8 + cq, split, acc[4 * j + 2 * hr], acc[4 * j + 2 * hr + 1]);
+        for (int q = 0; q < 4; ++q) {
+          const int xg = 2 * n0 + (q >> 1) * 256 + (q & 1) * 64;
+          if (q > 0) x_load(xg, 128, 2, y0);
+          x_wait();
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const int j = 8 * q + jj;
+#pragma unroll
+            for (int hr = 0; hr < 2; ++hr) {
+              const uint32_t ga = sa(hr, 0, jj, cq * 2), ua = sa(hr, 1, jj, cq * 2);
+              const float2 g2 = unpack_bf16x2(lds32(ga));
+              const float2 u2 = unpack_bf16x2(lds32(ua));
+              // d(act) is rounded to bf16 first, exactly like the unfused path that stores it
+              const float d0 = round_bf16(acc[4 * j + 2 * hr]), d1 = round_bf16(acc[4 * j + 2 * hr + 1]);
+              const float s0 = __fdividef(1.f, 1.f + __expf(-g2.x)), s1 = __fdividef(1.f, 1.f + __expf(-g2.y));
+              const float si0 = g2.x * s0, si1 = g2.y * s1;
+              sts32(ga, pack_bf16x2(d0 * u2.x * (s0 + si0 * (1.f - s0)), d1 * u2.y * (s1 + si1 * (1.f - s1))));
+              sts32(ua, pack_bf16x2(d0 * si0, d1 * si1));
+            }
+          }
+          pass_store(&tmC, p.c_cols, xg, 128, 2, y0, 0);
         }
       }
     }
+    if (issuer) tma_store_wait0();  // the kernel's last bulk stores are complete before its shared memory goes away
   }
 }
 
@@ -323,6 +426,26 @@ bool make_tmap_2d_bf16(CUtensorMap* out, const void* base, uint64_t inner, uint6
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS;
 }
+
+namespace {
+
+// 3-D fp32 tensor map over [outer2][outer][inner] with row stride ld and plane stride plane (elements), box {32, 64, 1}, 128B
+// swizzle: the split-K partial sums of EPI_F32, so that rows >= M of one split are clipped rather than written into the next
+bool make_tmap_3d_f32(CUtensorMap* out, const void* base, uint64_t inner, uint64_t outer, uint64_t outer2, uint64_t ld,
+                      uint64_t plane) {
+  EncodeTiledFn fn = get_encode_fn();
+  if (!fn) return false;
+  cuuint64_t gdim[3] = {inner, outer, outer2};
+  cuuint64_t gstride[2] = {ld * 4, plane * 4};
+  cuuint32_t box[3] = {32, 64, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<void*>(base), gdim, gstride, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS;
+}
+
+}  // namespace
 
 int gemm_num_sms() {
   static int n = 0;
@@ -378,6 +501,25 @@ cudaError_t launch(const GemmArgs& a, cudaStream_t s) {
     tA2 = tA;
     tB2 = tB;
   }
+  // epilogue tensor maps: C (and for the fused epilogues its second operand), boxes of 64 rows x 128 bytes
+  CUtensorMap tC, tX;
+  int c_cols = a.N, x_cols = 0;
+  if (EPI == EPI_SWIGLU_BWD) c_cols = 2 * a.N;  // d(gu) holds gate and up columns of every feature
+  if (EPI == EPI_F32) {
+    const int splits = a.split_k < 1 ? 1 : a.split_k;
+    ok &= make_tmap_3d_f32(&tC, a.C, a.N, a.M, splits, a.ldc, static_cast<uint64_t>(a.M) * a.ldc);
+  } else {
+    ok &= make_tmap_2d_bf16(&tC, a.C, c_cols, a.M, a.ldc, 64, 64);
+  }
+  if (EPI == EPI_BF16_ADD) {
+    x_cols = a.N;
+    ok &= make_tmap_2d_bf16(&tX, a.R, x_cols, a.M, a.ldr, 64, 64);
+  } else if (EPI == EPI_SWIGLU_FWD || EPI == EPI_SWIGLU_BWD) {
+    x_cols = EPI == EPI_SWIGLU_FWD ? a.N / 2 : 2 * a.N;  // act out / gu in
+    ok &= make_tmap_2d_bf16(&tX, a.aux, x_cols, a.M, a.ld_aux, 64, 64);
+  } else {
+    tX = tC;
+  }
   if (!ok) return cudaErrorInvalidValue;
 
   GemmKParams p;
@@ -407,10 +549,12 @@ cudaError_t launch(const GemmArgs& a, cudaStream_t s) {
   p.rope_inverse = a.rope_inverse;
   p.rope_pos = a.rope_pos;
   p.m_eff = p.split_k > 1 ? nullptr : a.m_eff;
+  p.c_cols = c_cols;
+  p.x_cols = x_cols;
   int total = p.m_tiles * p.n_tiles * p.split_k;
   int grid = total < gemm_num_sms() ? total : gemm_num_sms();
   if (grid <= 0) return cudaSuccess;
-  kern<<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, s>>>(tA, tB, tA2, tB2, p);
+  kern<<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, s>>>(tA, tB, tA2, tB2, tC, tX, p);
   return cudaGetLastError();
 }
 
@@ -455,11 +599,18 @@ cudaError_t gemm_bf16(const GemmArgs& a, cudaStream_t s) {
   if ((a.lda & 7) || (a.ldb & 7) || (reinterpret_cast<uintptr_t>(a.A) & 15) || (reinterpret_cast<uintptr_t>(a.B) & 15))
     return cudaErrorInvalidValue;
   if (a.K2 > 0 && ((a.lda2 & 7) || (a.ldb2 & 7) || !a.A2 || !a.B2)) return cudaErrorInvalidValue;
+  // the epilogue stores C (and loads R / reads or writes aux) through TMA as well
+  const int64_t c_align = a.epilogue == EPI_F32 ? 3 : 7;  // row stride in elements: a multiple of 16 bytes
+  if (!a.C || (a.ldc & c_align) || (reinterpret_cast<uintptr_t>(a.C) & 15)) return cudaErrorInvalidValue;
+  if (a.epilogue == EPI_BF16_ADD && ((a.ldr & 7) || (reinterpret_cast<uintptr_t>(a.R) & 15))) return cudaErrorInvalidValue;
+  if (a.epilogue == EPI_SWIGLU_FWD || a.epilogue == EPI_SWIGLU_BWD) {
+    if (!a.aux || (a.ld_aux & 7) || (reinterpret_cast<uintptr_t>(a.aux) & 15)) return cudaErrorInvalidValue;
+  }
   if (a.epilogue >= EPI_ROPE) {  // fused epilogues exist only for whole 256-column tiles
     if (a.a_mn_major || a.split_k > 1 || a.M <= 128 || !g_wide_tiles) return cudaErrorInvalidValue;
     if (a.epilogue == EPI_ROPE && (!a.rope_cs || a.rope_S <= 0 || (a.rope_cols & 255) || (a.N & 255))) return cudaErrorInvalidValue;
-    if (a.epilogue == EPI_SWIGLU_FWD && (!a.aux || (a.N & 255) || (a.ld_aux & 1) || (a.ldc & 1))) return cudaErrorInvalidValue;
-    if (a.epilogue == EPI_SWIGLU_BWD && (!a.aux || (a.N & 127) || (a.ld_aux & 1) || (a.ldc & 1))) return cudaErrorInvalidValue;
+    if (a.epilogue == EPI_SWIGLU_FWD && (a.N & 255)) return cudaErrorInvalidValue;
+    if (a.epilogue == EPI_SWIGLU_BWD && (a.N & 127)) return cudaErrorInvalidValue;
     return a.b_mn_major ? launch_fused<true>(a, s) : launch_fused<false>(a, s);
   }
   int bn = a.block_n;
