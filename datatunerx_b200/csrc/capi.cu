@@ -41,6 +41,26 @@ int32_t dtx_gemm_fused(const void* A, int64_t lda, const void* B, int64_t ldb, i
   return rc(gemm_bf16(g, S(stream)));
 }
 
+int32_t dtx_gemm_bias(const void* A, int64_t lda, const void* B, int64_t ldb, int32_t b_mn, const void* A2, int64_t lda2,
+                      const void* B2, int64_t ldb2, int32_t K2, void* C, int64_t ldc, void* aux, int64_t ld_aux, const void* rope_cs,
+                      int32_t rope_S, int32_t rope_cols, const void* rope_pos, int32_t M, int32_t N, int32_t K, int32_t epilogue,
+                      const void* bias, void* stream) {
+  if ((epilogue != EPI_BF16 && epilogue != EPI_ROPE) || !bias) return DTX_ERR_INVALID;
+  GemmArgs g;
+  g.A = static_cast<const bf16*>(A); g.lda = lda;
+  g.B = static_cast<const bf16*>(B); g.ldb = ldb; g.b_mn_major = b_mn;
+  g.A2 = static_cast<const bf16*>(A2); g.lda2 = lda2; g.B2 = static_cast<const bf16*>(B2); g.ldb2 = ldb2; g.K2 = K2;
+  g.C = C; g.ldc = ldc; g.aux = aux; g.ld_aux = ld_aux;
+  g.rope_cs = static_cast<const float2*>(rope_cs); g.rope_S = rope_S; g.rope_cols = rope_cols;
+  g.rope_pos = static_cast<const int32_t*>(rope_pos);
+  g.M = M; g.N = N; g.K = K; g.epilogue = epilogue; g.bias = static_cast<const bf16*>(bias);
+  return rc(gemm_bf16(g, S(stream)));
+}
+
+int32_t dtx_bias_grad(const void* dy, int64_t ld, int32_t M, int32_t n, void* db, int32_t accumulate, void* stream) {
+  return rc(bias_grad(static_cast<const bf16*>(dy), ld, M, n, static_cast<bf16*>(db), accumulate, S(stream)));
+}
+
 int32_t dtx_set_option(const char* name, int32_t value) {
   if (!name) return DTX_ERR_INVALID;
   if (strcmp(name, "gemm_pair_kernel") == 0) {

@@ -745,6 +745,38 @@ __global__ void rmsnorm_dw_stage2(const float* __restrict__ part, int d, bf16* _
   if (accumulate) s += __bfloat162float(dw[c]);
   dw[c] = __float2bfloat16_rn(s);
 }
+// bias gradient: block b sums columns [64 b, +64) over all rows - 256 threads = 32 column pairs x 8 row lanes; lane r adds rows
+// r, r + 8, ... in order, then the eight lane sums are added in a fixed tree (deterministic: no atomics, no order that
+// depends on the launch)
+constexpr int BG_LANES = 8;
+__global__ void __launch_bounds__(256) bias_grad_kernel(const bf16* __restrict__ dy, long long ld, int M, int n, bf16* __restrict__ db,
+                                                        int accumulate) {
+  __shared__ float2 sh[BG_LANES][32];
+  const int cp = threadIdx.x & 31, lane_r = threadIdx.x >> 5;
+  const int c = blockIdx.x * 64 + 2 * cp;
+  float2 acc = make_float2(0.f, 0.f);
+  if (c < n)
+    for (int m = lane_r; m < M; m += BG_LANES) {
+      const float2 v = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(dy + static_cast<size_t>(m) * ld + c));
+      acc.x += v.x;
+      acc.y += v.y;
+    }
+  sh[lane_r][cp] = acc;
+  __syncthreads();
+  if (lane_r == 0 && c < n) {
+    float2 s01 = make_float2(sh[0][cp].x + sh[1][cp].x, sh[0][cp].y + sh[1][cp].y);
+    float2 s23 = make_float2(sh[2][cp].x + sh[3][cp].x, sh[2][cp].y + sh[3][cp].y);
+    float2 s45 = make_float2(sh[4][cp].x + sh[5][cp].x, sh[4][cp].y + sh[5][cp].y);
+    float2 s67 = make_float2(sh[6][cp].x + sh[7][cp].x, sh[6][cp].y + sh[7][cp].y);
+    float x = (s01.x + s23.x) + (s45.x + s67.x), y = (s01.y + s23.y) + (s45.y + s67.y);
+    if (accumulate) {
+      x += __bfloat162float(db[c]);
+      y += __bfloat162float(db[c + 1]);
+    }
+    db[c] = __float2bfloat16_rn(x);
+    db[c + 1] = __float2bfloat16_rn(y);
+  }
+}
 __global__ void embedding_bwd_kernel(const int32_t* __restrict__ ids, const bf16* __restrict__ dx, float* __restrict__ dE, int d, int vocab) {
   const int m = blockIdx.x;
   const int id = ids[m];
@@ -999,6 +1031,13 @@ cudaError_t rmsnorm_dw(const bf16* dy, const bf16* x, const float* rstd, int M, 
                        cudaStream_t s) {
   rmsnorm_dw_stage1<<<dim3((d + 63) / 64, NDW_ROWBLOCKS), 256, 0, s>>>(dy, x, rstd, M, d, scratch);
   rmsnorm_dw_stage2<<<(d + 255) / 256, 256, 0, s>>>(scratch, d, dw, accumulate);
+  return cudaGetLastError();
+}
+cudaError_t bias_grad(const bf16* dy, int64_t ld, int M, int n, bf16* db, int accumulate, cudaStream_t s) {
+  if (!dy || !db || M <= 0 || n <= 0 || (n & 1) || (ld & 1) || ld < n || (reinterpret_cast<uintptr_t>(dy) & 3) ||
+      (reinterpret_cast<uintptr_t>(db) & 3))
+    return cudaErrorInvalidValue;
+  bias_grad_kernel<<<(n + 63) / 64, 256, 0, s>>>(dy, ld, M, n, db, accumulate);
   return cudaGetLastError();
 }
 cudaError_t embedding_bwd(const int32_t* ids, const bf16* dx, float* dE32, int M, int d, int vocab, cudaStream_t s) {

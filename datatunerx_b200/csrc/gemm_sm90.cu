@@ -49,6 +49,7 @@ struct GemmKParams {
   const int32_t* rope_pos;  // optional per-row position (packed ragged batches); null: row % rope_S
   const int32_t* m_eff;  // device-side row count; 256-row blocks that start at or beyond it are skipped
   int c_cols, x_cols;    // inner extents of the tmC / tmX tensor maps: output boxes at or beyond them are not issued
+  const bf16* bias;      // BIAS kernels: bf16 [N], added to the accumulator before rounding / rotary
 };
 
 template <int BN>
@@ -62,19 +63,26 @@ struct GemmCfg {
   static constexpr int STG_BYTES = 2 * 2 * BOX_BYTES;    // two boxes per consumer warpgroup
   // 230 656 of the 232 448 bytes a block may opt into
   static constexpr int SMEM_BYTES = RING_BYTES + STG_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  // BIAS kernels: each consumer warpgroup stages the tile's BN bias values behind the barriers (231 680 bytes at BN = 256)
+  static constexpr int BIAS_BYTES = 2 * BN * 2;
 };
 
 __device__ __forceinline__ float round_bf16(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
 
 // tmC: the output C (fp32: 3-D [split][M][N] with box {32, 64, 1}; bf16: 2-D with box {64, 64});
 // tmX: the second operand of the epilogue (R of EPI_BF16_ADD, act of EPI_SWIGLU_FWD, gu of EPI_SWIGLU_BWD), bf16 box {64, 64}
-template <int BN, bool A_MN, bool B_MN, int EPI>
+// BIAS (EPI_BF16 / EPI_ROPE only): p.bias[n] is added to column n of the fp32 accumulator before the rounding or the rotary.  Each
+// consumer warpgroup copies the tile's slice into its own shared-memory row at the start of the tile (one coalesced load per thread,
+// hidden under the main loop); the first pass_begin() barrier of the epilogue orders it before the reads, the last pass_store()
+// barrier of the previous tile orders the previous tile's reads before it.
+template <int BN, bool A_MN, bool B_MN, int EPI, bool BIAS = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
             const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
             const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmX, const GemmKParams p) {
   using Cfg = GemmCfg<BN>;
   static_assert(EPI < EPI_ROPE || BN == 256, "the fused epilogues pair columns 64 / 128 apart inside one 256-column tile");
+  static_assert(!BIAS || EPI == EPI_BF16 || EPI == EPI_ROPE, "the bias is added by the EPI_BF16 and EPI_ROPE epilogues only");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::RING_BYTES + Cfg::STG_BYTES);
@@ -172,6 +180,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     uint8_t* stg = smem + Cfg::RING_BYTES + cw * 2 * Cfg::BOX_BYTES;
     const uint32_t stg_u = smem_u32(stg);
     uint32_t x_phase = 0;
+    bf16* bias_s = reinterpret_cast<bf16*>(smem + Cfg::RING_BYTES + Cfg::STG_BYTES + 256) + cw * BN;
+    // bias of columns 8 j + cq, + 1 of the tile
+    auto bias2 = [&](int j) -> float2 { return __bfloat1622float2(reinterpret_cast<const __nv_bfloat162*>(bias_s)[4 * j + (cq >> 1)]); };
     int stage = 0;
     uint32_t phase = 0;
     float acc[BN / 2];
@@ -224,6 +235,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       if (dead(m_blk)) continue;
       const int m0 = m_blk * BM, n0 = n_blk * BN;
       const int y0 = m0 + cw * 64;  // first row of this warpgroup's slice
+      if (BIAS)
+        for (int c = threadIdx.x & 127; c < BN; c += 128) bias_s[c] = n0 + c < p.N ? __ldg(p.bias + n0 + c) : __float2bfloat16_rn(0.f);
       int prev = -1;
       for (int kb = kb_begin; kb < kb_end; ++kb) {
         mbar_wait(&full_bar[stage], phase);
@@ -269,6 +282,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             for (int hr = 0; hr < 2; ++hr) {
               const uint32_t a = sa(hr, jj >> 3, jj & 7, cq * 2);
               float v0 = acc[4 * j + 2 * hr], v1 = acc[4 * j + 2 * hr + 1];
+              if (BIAS) {
+                const float2 b = bias2(j);
+                v0 += b.x;
+                v1 += b.y;
+              }
               if (EPI == EPI_BF16_ADD) {  // the residual tile sits where the output goes
                 const float2 rr = unpack_bf16x2(lds32(a));
                 v0 += rr.x;
@@ -312,6 +330,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 #pragma unroll
             for (int hr = 0; hr < 2; ++hr) {
               float lo[2] = {acc[4 * jl + 2 * hr], acc[4 * jl + 2 * hr + 1]}, hi[2] = {acc[4 * jh + 2 * hr], acc[4 * jh + 2 * hr + 1]};
+              if (BIAS) {  // HF order: q = x W^T + b, then the rotary
+                const float2 bl = bias2(jl), bh = bias2(jh);
+                lo[0] += bl.x;
+                lo[1] += bl.y;
+                hi[0] += bh.x;
+                hi[1] += bh.y;
+              }
               if (rot) {
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
@@ -479,12 +504,13 @@ struct DeviceOnce {
 int g_wide_tiles = 1;
 int g_group_m = GROUP_M;
 
-template <int BN, bool A_MN, bool B_MN, int EPI>
+template <int BN, bool A_MN, bool B_MN, int EPI, bool BIAS = false>
 cudaError_t launch(const GemmArgs& a, cudaStream_t s) {
   using Cfg = GemmCfg<BN>;
-  auto kern = gemm_kernel<BN, A_MN, B_MN, EPI>;
+  constexpr int SMEM = Cfg::SMEM_BYTES + (BIAS ? Cfg::BIAS_BYTES : 0);
+  auto kern = gemm_kernel<BN, A_MN, B_MN, EPI, BIAS>;
   static DeviceOnce attr;  // the attribute is per device: a second trainer on another GPU of the same process needs it too
-  if (cudaError_t e = attr.run([&] { return cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES); });
+  if (cudaError_t e = attr.run([&] { return cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM); });
       e != cudaSuccess)
     return e;
   CUtensorMap tA, tB, tA2, tB2;
@@ -551,10 +577,11 @@ cudaError_t launch(const GemmArgs& a, cudaStream_t s) {
   p.m_eff = p.split_k > 1 ? nullptr : a.m_eff;
   p.c_cols = c_cols;
   p.x_cols = x_cols;
+  p.bias = a.bias;
   int total = p.m_tiles * p.n_tiles * p.split_k;
   int grid = total < gemm_num_sms() ? total : gemm_num_sms();
   if (grid <= 0) return cudaSuccess;
-  kern<<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, s>>>(tA, tB, tA2, tB2, tC, tX, p);
+  kern<<<grid, GEMM_THREADS, SMEM, s>>>(tA, tB, tA2, tB2, tC, tX, p);
   return cudaGetLastError();
 }
 
@@ -570,6 +597,7 @@ cudaError_t launch_epi(const GemmArgs& a, cudaStream_t s) {
 
 template <bool B_MN>
 cudaError_t launch_fused(const GemmArgs& a, cudaStream_t s) {
+  if (a.bias) return a.epilogue == EPI_ROPE ? launch<256, false, B_MN, EPI_ROPE, true>(a, s) : cudaErrorInvalidValue;
   switch (a.epilogue) {
     case EPI_ROPE: return launch<256, false, B_MN, EPI_ROPE>(a, s);
     case EPI_SWIGLU_FWD: return launch<256, false, B_MN, EPI_SWIGLU_FWD>(a, s);
@@ -580,6 +608,9 @@ cudaError_t launch_fused(const GemmArgs& a, cudaStream_t s) {
 
 template <int BN>
 cudaError_t launch_major(const GemmArgs& a, cudaStream_t s) {
+  if (a.bias) {  // EPI_BF16 with a K-major A (checked by gemm_bf16)
+    return a.b_mn_major ? launch<BN, false, true, EPI_BF16, true>(a, s) : launch<BN, false, false, EPI_BF16, true>(a, s);
+  }
   if (!a.a_mn_major && !a.b_mn_major) return launch_epi<BN, false, false>(a, s);
   if (!a.a_mn_major && a.b_mn_major) return launch_epi<BN, false, true>(a, s);
   if (a.a_mn_major && a.b_mn_major) return launch_epi<BN, true, true>(a, s);
@@ -595,6 +626,8 @@ cudaError_t gemm_bf16(const GemmArgs& a, cudaStream_t s) {
   if (a.M <= 0 || a.N <= 0 || a.K <= 0) return cudaErrorInvalidValue;
   if (a.split_k > 1 && a.epilogue != EPI_F32) return cudaErrorInvalidValue;
   if (a.epilogue == EPI_BF16_ADD && a.R == nullptr) return cudaErrorInvalidValue;
+  // bias variants: the plain bf16 and the RoPE epilogue, K-major A, one split
+  if (a.bias && ((a.epilogue != EPI_BF16 && a.epilogue != EPI_ROPE) || a.a_mn_major || a.split_k > 1)) return cudaErrorInvalidValue;
   // TMA needs 16-byte aligned bases and row strides
   if ((a.lda & 7) || (a.ldb & 7) || (reinterpret_cast<uintptr_t>(a.A) & 15) || (reinterpret_cast<uintptr_t>(a.B) & 15))
     return cudaErrorInvalidValue;

@@ -36,6 +36,8 @@ struct GemmArgs {
   void* aux = nullptr; int64_t ld_aux = 0;             // EPI_SWIGLU_FWD: act out; EPI_SWIGLU_BWD: gu in (ld = 2F)
   const float2* rope_cs = nullptr; int rope_S = 0, rope_cols = 0, rope_inverse = 0;  // EPI_ROPE
   const int32_t* rope_pos = nullptr;  // EPI_ROPE, optional [M]: position of every row inside its sequence (packed ragged batches); null: row % rope_S
+  // optional bf16 [N] (EPI_BF16 / EPI_ROPE only, K-major A): added to the fp32 accumulator before rounding / rotary (q|k|v biases)
+  const bf16* bias = nullptr;
   int M = 0, N = 0, K = 0;
   // optional device-side row count (<= M): 256-row blocks of tiles that start at or beyond it are skipped (rows up to the
   // end of the last live block are still computed).  Lets the lm_head GEMMs run over the unmasked tokens only without a
@@ -180,6 +182,8 @@ cudaError_t rmsnorm_dw(const bf16* dy, const bf16* x, const float* rstd, int M, 
                        cudaStream_t s);
 // embedding gradient: dE32[ids[m], :] += dx[m, :]  (fp32 atomics: the one reduction of the step whose order is not fixed)
 cudaError_t embedding_bwd(const int32_t* ids, const bf16* dx, float* dE32, int M, int d, int vocab, cudaStream_t s);
+// bias gradient: db[c] (+)= sum_m dy[m, c] (row stride ld; fp32 per-thread partials summed in a fixed order, no atomics)
+cudaError_t bias_grad(const bf16* dy, int64_t ld, int M, int n, bf16* db, int accumulate, cudaStream_t s);
 // dst[i] = (accumulate ? dst[i] : 0) + src[i]   fp32 -> bf16
 cudaError_t add_f32_into_bf16(const float* src, bf16* dst, int64_t n, int accumulate, cudaStream_t s);
 // *out (+)= sum g[i]^2 over a bf16 buffer (two-stage, fixed order; first = 1 overwrites)

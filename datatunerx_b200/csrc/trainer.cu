@@ -148,6 +148,7 @@ __global__ void lora_shadow_kernel(ShadowArgs a) {
 struct Layer {
   // wgu: [2F, d] in the GU-interleaved layout (128 gate rows | 128 up rows per 128 features)
   bf16 *wqkv = nullptr, *wo = nullptr, *wgu = nullptr, *wdown = nullptr, *norm1 = nullptr, *norm2 = nullptr;
+  bf16* bias = nullptr;  // dtx_model_ext.qkv_bias: [W] q|k|v biases in the row order of wqkv (bf16 also under NF4), else null
   bf16 *a_cat = nullptr, *b_ext = nullptr;                                               // shadows
   bf16 *h1 = nullptr, *t = nullptr, *qkv = nullptr, *attn = nullptr, *x_mid = nullptr, *gu = nullptr;  // saved
   bf16* hd = nullptr;  // LoRA dropout only: [M, nt*d] dropped copies of h1, one per target (peft: one nn.Dropout per module)
@@ -179,6 +180,7 @@ using namespace dtx;
 
 struct dtx_trainer {
   dtx_model_cfg mc{};
+  dtx_model_ext ext{};          // all zero: plain Llama-2 / Mistral
   dtx_train_cfg tc{};
   int device = 0, rank = 0, world = 1;
   cudaStream_t stream = nullptr;
@@ -236,6 +238,8 @@ struct dtx_trainer {
   // in place (NCCL, on a side stream, as soon as the backward pass has finished the layer), the fp32 master weights and Adam
   // moments exist for the owned slices only (ZeRO-1 style), and the updated bf16 slices are all-gathered in place.
   bool full = false;
+  bool qkv_bias = false;        // q|k|v biases (Qwen2): Layer::bias; full-parameter SFT keeps them at off_bias of the layer block
+  int64_t off_bias = 0;
   int64_t layer_elems = 0, glob_elems = 0;
   int64_t off_wo = 0, off_wgu = 0, off_wdown = 0, off_n1 = 0, off_n2 = 0, goff_lm = 0, goff_nf = 0, layer_used = 0, glob_used = 0;
   bf16 *w_flat = nullptr, *g_flat = nullptr;
@@ -262,6 +266,7 @@ struct dtx_trainer {
   // which base tensors have been uploaded: [0] embed, [1] lm_head, [2] final norm, then 9 per layer
   // (q, k, v, o, gate, up, down, norm1, norm2); a step with a hole in this map would train on uninitialised memory
   std::vector<uint8_t> loaded;
+  std::vector<uint8_t> bias_loaded;  // qkv_bias: q, k, v bias of every layer
   bool all_random = false;
   bool have_lora = false;
   cudaEvent_t ev_fb = nullptr, ev_ar = nullptr;
@@ -328,6 +333,11 @@ struct dtx_trainer {
         else snprintf(buf, n, "model.layers.%zu.%s.weight", (i - 3) / 9, per[(i - 3) % 9]);
         return buf;
       }
+    for (size_t i = 0; i < bias_loaded.size(); ++i)
+      if (!bias_loaded[i]) {
+        snprintf(buf, n, "model.layers.%zu.%s.bias", i / 3, per[i % 3]);
+        return buf;
+      }
     return nullptr;
   }
 };
@@ -379,6 +389,39 @@ int pick_split(int n_sms, int m_tiles, int kb_total) {
   return s;
 }
 
+// fp32 inverse frequencies of the rotary table (half = head_dim / 2 values) in HF's operation order, so that the table is bitwise
+// the one transformers builds: the default type is 1 / theta^(2i/D) (powf), linear divides it by the factor
+// (_compute_linear_scaling_rope_parameters), llama3 follows _compute_llama3_parameters - wavelen = 2 pi / inv_freq (torch
+// evaluates a scalar over a tensor as reciprocal times scalar), wavelengths below original_max_pos / high_freq_factor keep their
+// frequency, those above original_max_pos / low_freq_factor are divided by the factor, the band between is interpolated.
+void rope_inv_freq(const dtx_model_cfg& mc, const dtx_model_ext& ext, float* out) {
+  const int half = mc.head_dim / 2;
+  for (int i = 0; i < half; ++i) {
+    const float base = 1.0f / powf(mc.rope_theta, static_cast<float>(2 * i) / static_cast<float>(mc.head_dim));
+    float f = base;
+    if (ext.rope_type == DTX_ROPE_LINEAR) {
+      f = base / ext.rope_factor;
+    } else if (ext.rope_type == DTX_ROPE_LLAMA3) {
+      const double old_len = ext.rope_original_max_pos;
+      const float low_wavelen = static_cast<float>(old_len / ext.rope_low_freq_factor);
+      const float high_wavelen = static_cast<float>(old_len / ext.rope_high_freq_factor);
+      const float factor = ext.rope_factor;
+      const float wavelen = (1.0f / base) * static_cast<float>(2.0 * M_PI);
+      const float scaled = wavelen > low_wavelen ? base / factor : base;
+      if (!(wavelen < high_wavelen) && !(wavelen > low_wavelen)) {
+        const float smooth = ((1.0f / wavelen) * static_cast<float>(old_len) - ext.rope_low_freq_factor) /
+                             static_cast<float>(static_cast<double>(ext.rope_high_freq_factor) - ext.rope_low_freq_factor);
+        const float a = (1.0f - smooth) * scaled;
+        const float b = smooth * scaled;
+        f = a / factor + b;
+      } else {
+        f = scaled;
+      }
+    }
+    out[i] = f;
+  }
+}
+
 int create_buffers(dtx_trainer* t) {
   const dtx_model_cfg& mc = t->mc;
   const dtx_train_cfg& tc = t->tc;
@@ -395,6 +438,10 @@ int create_buffers(dtx_trainer* t) {
     t->off_n1 = t->off_wdown + d * F;
     t->off_n2 = t->off_n1 + d;
     t->layer_used = t->off_n2 + d;
+    if (t->qkv_bias) {  // no weight decay either (HF get_decay_parameter_names excludes "bias"): inside the block's no-decay tail
+      t->off_bias = t->layer_used;
+      t->layer_used += W;
+    }
     t->layer_elems = pad(t->layer_used);
     t->goff_lm = V * d;
     t->goff_nf = 2 * V * d;
@@ -423,6 +470,7 @@ int create_buffers(dtx_trainer* t) {
   }
   t->base_bytes = static_cast<int64_t>((2 * V * d + d) * sizeof(bf16));
   t->loaded.assign(3 + 9 * L, 0);
+  t->bias_loaded.assign(t->qkv_bias ? 3 * L : 0, 0);
   t->layers.resize(L);
   t->xs.resize(L + 1);
   for (size_t l = 0; l <= L; ++l) ok = ok && t->alloc(&t->xs[l], M * d);
@@ -432,13 +480,15 @@ int create_buffers(dtx_trainer* t) {
       bf16* blk = t->w_flat + l * t->layer_elems;
       y.wqkv = blk; y.wo = blk + t->off_wo; y.wgu = blk + t->off_wgu; y.wdown = blk + t->off_wdown;
       y.norm1 = blk + t->off_n1; y.norm2 = blk + t->off_n2;
+      if (t->qkv_bias) y.bias = blk + t->off_bias;
     } else {
       ok = ok && t->alloc(&y.wqkv, W * d) && t->alloc(&y.wo, d * d) && t->alloc(&y.wgu, 2 * F * d) &&
            t->alloc(&y.wdown, d * F) && t->alloc(&y.norm1, d) && t->alloc(&y.norm2, d);
+      if (t->qkv_bias) ok = ok && t->alloc(&y.bias, W);
       y.a_cat = t->a_cat_all + l * RP * KA;
       y.b_ext = t->b_ext_all + l * W * RP;
     }
-    t->base_bytes += static_cast<int64_t>((W * d + d * d + 3 * F * d + 2 * d) * sizeof(bf16));
+    t->base_bytes += static_cast<int64_t>((W * d + d * d + 3 * F * d + 2 * d + (t->qkv_bias ? W : 0)) * sizeof(bf16));
     if (t->recompute == RECOMPUTE_LAYER && l > 0) {  // one saved set, refilled layer by layer
       const Layer& y0 = t->layers[0];
       y.h1 = y0.h1; y.t = y0.t; y.hd = y0.hd; y.qkv = y0.qkv; y.attn = y0.attn; y.x_mid = y0.x_mid; y.gu = y0.gu;
@@ -485,15 +535,16 @@ int create_buffers(dtx_trainer* t) {
   ok = ok && t->alloc(&t->rope_cs_t, static_cast<size_t>(tc.seq_len) * (mc.head_dim / 2));
   if (!ok) return DTX_ERR_CUDA;
   if (t->dry) return DTX_OK;
-  // rotary table in double precision (HF LlamaRotaryEmbedding: inv_freq = theta^(-2i/D))
+  // rotary table in double precision (HF LlamaRotaryEmbedding; inverse frequencies of the model's rope type)
   {
     const int half = mc.head_dim / 2;
+    std::vector<float> inv_freq(half);
+    rope_inv_freq(mc, t->ext, inv_freq.data());
     std::vector<float2> cs(static_cast<size_t>(tc.seq_len) * half);
     for (int pos = 0; pos < tc.seq_len; ++pos)
       for (int i = 0; i < half; ++i) {
         // HF computes inv_freq and the angle in fp32; reproduce that rounding, then take cos/sin accurately
-        const float inv_freq = 1.0f / powf(mc.rope_theta, static_cast<float>(2 * i) / static_cast<float>(mc.head_dim));
-        const float ang = static_cast<float>(pos) * inv_freq;
+        const float ang = static_cast<float>(pos) * inv_freq[i];
         cs[static_cast<size_t>(pos) * half + i] = make_float2(static_cast<float>(cos(static_cast<double>(ang))),
                                                               static_cast<float>(sin(static_cast<double>(ang))));
       }
@@ -677,6 +728,7 @@ int layer_fwd(dtx_trainer* t, int l, int phase, bool backward) {
     g.A = y.h1; g.lda = d; g.B = wqkv; g.ldb = d;
     if (lora) { g.A2 = y.t; g.lda2 = RP; g.B2 = y.b_ext; g.ldb2 = RP; g.K2 = RP; }
     g.C = y.qkv; g.ldc = W; g.M = M; g.N = W; g.K = d; g.epilogue = EPI_BF16;
+    g.bias = y.bias;  // q|k|v biases (Qwen2): added to the accumulator before the rounding / the rotary
     if (fused) {  // rotary embedding of q and k applied to the fp32 accumulator in the epilogue
       g.epilogue = EPI_ROPE; g.rope_cs = t->rope_cs; g.rope_S = S; g.rope_cols = t->dq + t->dkv;
       g.rope_pos = t->packed ? t->d_pos : nullptr;  // packed batch: a row's position is its offset inside its own sequence
@@ -862,6 +914,7 @@ int fwd_bwd(dtx_trainer* t, bool backward) {
       CK(gemm_bf16(g, s), 1);
     }
     if (t->full) CK(dw_gemm(t->dqkv, W, y.h1, d, gl_w), 1);  // dWqkv = dqkv^T * h1 (dqkv already carries the inverse rotary)
+    if (t->full && t->qkv_bias) CK(bias_grad(t->dqkv, W, M, W, gl_w + t->off_bias, accumulate, s), 1);  // db = column sums of dqkv
     // LoRA: layer 0's input gradient has no consumer (the embedding is frozen, SURVEY §8a): its dh1 GEMM, the dropout-branch
     // gradient and the norm-1 backward are skipped.  Full-parameter SFT trains the embedding and needs them.
     const bool need_dx = l > 0 || t->full;
@@ -1297,9 +1350,30 @@ int check_cfg(const dtx_model_cfg* mc, const dtx_train_cfg* tc) {
   return DTX_OK;
 }
 
+// checks of the model-family extensions (host only; the message goes to g_error)
+int check_ext(const dtx_model_ext* ext) {
+  if (!ext) return DTX_OK;
+  auto bad = [&](const char* m) {
+    g_error = m;
+    return DTX_ERR_INVALID;
+  };
+  if (ext->qkv_bias != 0 && ext->qkv_bias != 1) return bad("qkv_bias must be 0 or 1");
+  if (ext->rope_type < DTX_ROPE_DEFAULT || ext->rope_type > DTX_ROPE_LLAMA3)
+    return bad("rope_type must be DTX_ROPE_DEFAULT, DTX_ROPE_LINEAR or DTX_ROPE_LLAMA3 (yarn, dynamic, longrope are not implemented)");
+  if (ext->rope_type != DTX_ROPE_DEFAULT && !(ext->rope_factor > 0.0f)) return bad("rope_factor must be > 0");
+  if (ext->rope_type == DTX_ROPE_LLAMA3) {
+    if (!(ext->rope_low_freq_factor > 0.0f) || !(ext->rope_low_freq_factor < ext->rope_high_freq_factor))
+      return bad("llama3 rope scaling needs 0 < low_freq_factor < high_freq_factor");
+    if (ext->rope_original_max_pos <= 0) return bad("llama3 rope scaling needs original_max_position_embeddings > 0");
+  }
+  return DTX_OK;
+}
+
 // shapes and adapter geometry derived from the configuration (host only)
-void setup_dims(dtx_trainer* t, const dtx_model_cfg* mc, const dtx_train_cfg* tc, int world) {
+void setup_dims(dtx_trainer* t, const dtx_model_cfg* mc, const dtx_model_ext* ext, const dtx_train_cfg* tc, int world) {
   t->mc = *mc;
+  if (ext) t->ext = *ext;
+  t->qkv_bias = t->ext.qkv_bias != 0;
   t->tc = *tc;
   t->world = world;
   t->M = tc->micro_batch * tc->seq_len;
@@ -1337,9 +1411,9 @@ void setup_dims(dtx_trainer* t, const dtx_model_cfg* mc, const dtx_train_cfg* tc
 
 // device bytes create_buffers() allocates for this configuration and activation layout: the same function in a sizing run,
 // so that the plan cannot drift from the allocation (n_sms sizes the split-K partial buffers of the adapter gradients)
-int64_t planned_bytes(const dtx_model_cfg* mc, const dtx_train_cfg* tc, int world, int n_sms, int layout) {
+int64_t planned_bytes(const dtx_model_cfg* mc, const dtx_model_ext* ext, const dtx_train_cfg* tc, int world, int n_sms, int layout) {
   dtx_trainer p;
-  setup_dims(&p, mc, tc, world);
+  setup_dims(&p, mc, ext, tc, world);
   p.n_sms = n_sms;
   p.dry = true;
   p.recompute = layout;
@@ -1388,12 +1462,35 @@ int32_t dtx_get_nccl_unique_id(void* out128) {
 
 int32_t dtx_trainer_create(const dtx_model_cfg* mc, const dtx_train_cfg* tc, int32_t device, int32_t rank, int32_t world,
                            const void* nccl_unique_id, dtx_trainer** out) {
+  return dtx_trainer_create_ext(mc, nullptr, tc, device, rank, world, nccl_unique_id, out);
+}
+
+int32_t dtx_rope_inv_freq(const dtx_model_cfg* mc, const dtx_model_ext* ext, float* out) {
+  if (!mc || !out) {
+    g_error = "rope_inv_freq: null argument";
+    return DTX_ERR_INVALID;
+  }
+  if (mc->head_dim <= 0 || mc->head_dim % 2) {
+    g_error = "rope_inv_freq: head_dim must be a positive even number";
+    return DTX_ERR_INVALID;
+  }
+  int rc = check_ext(ext);
+  if (rc) return rc;
+  dtx_model_ext e{};
+  if (ext) e = *ext;
+  rope_inv_freq(*mc, e, out);
+  return DTX_OK;
+}
+
+int32_t dtx_trainer_create_ext(const dtx_model_cfg* mc, const dtx_model_ext* ext, const dtx_train_cfg* tc, int32_t device,
+                               int32_t rank, int32_t world, const void* nccl_unique_id, dtx_trainer** out) {
   if (!mc || !tc || !out) {
     g_error = "null argument";
     return DTX_ERR_INVALID;
   }
   *out = nullptr;
   int rc = check_cfg(mc, tc);
+  if (rc == DTX_OK) rc = check_ext(ext);
   if (rc) return rc;
   if (world < 1 || rank < 0 || rank >= world) {
     g_error = "bad rank/world";
@@ -1416,7 +1513,7 @@ int32_t dtx_trainer_create(const dtx_model_cfg* mc, const dtx_train_cfg* tc, int
     return DTX_ERR_CUDA;
   }
   dtx_trainer* t = new dtx_trainer();
-  setup_dims(t, mc, tc, world);
+  setup_dims(t, mc, ext, tc, world);
   t->device = device;
   t->rank = rank;
   if (prop.multiProcessorCount > 0) t->n_sms = prop.multiProcessorCount;
@@ -1431,8 +1528,8 @@ int32_t dtx_trainer_create(const dtx_model_cfg* mc, const dtx_train_cfg* tc, int
       delete t;
       return DTX_ERR_CUDA;
     }
-    const int64_t keep = planned_bytes(mc, tc, world, t->n_sms, KEEP_ALL);
-    const int64_t layer = planned_bytes(mc, tc, world, t->n_sms, RECOMPUTE_LAYER);
+    const int64_t keep = planned_bytes(mc, ext, tc, world, t->n_sms, KEEP_ALL);
+    const int64_t layer = planned_bytes(mc, ext, tc, world, t->n_sms, RECOMPUTE_LAYER);
     const int64_t avail = static_cast<int64_t>(free_b) - kHeadroomBytes;
     if (keep <= avail) {
       t->recompute = KEEP_ALL;
@@ -1589,6 +1686,18 @@ int32_t dtx_load_tensor(dtx_trainer* t, const char* name, const void* host, int3
     CKM(cudaStreamSynchronize(t->stream));
     return DTX_OK;
   }
+  {  // q|k|v biases [dq] / [dkv]: one [W] vector per layer in the row order of wqkv (bf16 also under NF4, like bitsandbytes)
+    static const char* keys[3] = {"self_attn.q_proj.bias", "self_attn.k_proj.bias", "self_attn.v_proj.bias"};
+    const int64_t row0[3] = {0, dq, dq + dkv}, n[3] = {dq, dkv, dkv};
+    for (int i = 0; i < 3; ++i) {
+      if (!strstr(rest, keys[i])) continue;
+      if (!t->qkv_bias) return t->fail(DTX_ERR_INVALID, "%s: this trainer was created without q/k/v biases (dtx_model_ext.qkv_bias)", name);
+      if (nd != 1 || rows != n[i]) return t->fail(DTX_ERR_INVALID, "%s: expected [%lld]", name, (long long)n[i]);
+      int rc = upload(y.bias + row0[i], n[i]);
+      if (rc == DTX_OK) t->bias_loaded[3 * static_cast<size_t>(layer) + i] = 1;
+      return rc;
+    }
+  }
   if (t->quant4 && !strstr(rest, "layernorm"))
     return t->fail(DTX_ERR_STATE, "%s: the base weights are already NF4-packed; load tensors before dtx_quantize_base", name);
   // gate/up rows go to the GU-interleaved layout: 128 gate rows, then the 128 up rows of the same features, ...
@@ -1642,10 +1751,12 @@ int32_t dtx_init_random_weights(dtx_trainer* t, uint64_t seed) {
     CK(fill_normal_bf16(y.wdown, d * F, 0.02f, ++k, s), 1);
     CK(fill_const_bf16(y.norm1, d, 1.0f, s), 1);
     CK(fill_const_bf16(y.norm2, d, 1.0f, s), 1);
+    if (y.bias) CK(fill_const_bf16(y.bias, t->W, 0.0f, s), 1);  // HF _init_weights zeroes Linear biases
   }
   cudaError_t e = cudaStreamSynchronize(s);
   if (e != cudaSuccess) return t->fail(DTX_ERR_CUDA, "init_random_weights: %s", cudaGetErrorString(e));
   std::fill(t->loaded.begin(), t->loaded.end(), 1);
+  std::fill(t->bias_loaded.begin(), t->bias_loaded.end(), 1);
   return DTX_OK;
 }
 
@@ -2008,6 +2119,14 @@ int32_t dtx_export_weight(dtx_trainer* t, const char* name, void* host_out, int6
   };
   for (const Slot& sl : slots)
     if (strstr(rest, sl.key)) return copy(blk + sl.off, sl.n);
+  if (t->qkv_bias) {
+    const Slot bias_slots[] = {
+        {"self_attn.q_proj.bias", t->off_bias, dq}, {"self_attn.k_proj.bias", t->off_bias + dq, dkv},
+        {"self_attn.v_proj.bias", t->off_bias + dq + dkv, dkv},
+    };
+    for (const Slot& sl : bias_slots)
+      if (strstr(rest, sl.key)) return copy(blk + sl.off, sl.n);
+  }
   return t->fail(DTX_ERR_INVALID, "unknown tensor name %s", name);
 }
 
@@ -2016,6 +2135,10 @@ int32_t dtx_recompute(const dtx_trainer* t) { return t ? t->recompute : DTX_ERR_
 int64_t dtx_device_bytes(const dtx_trainer* t) { return t ? static_cast<int64_t>(t->bytes_allocated) : 0; }
 
 int32_t dtx_plan_device_bytes(const dtx_model_cfg* mc, const dtx_train_cfg* tc, int32_t world, int32_t layout, int64_t* bytes_out) {
+  return dtx_plan_device_bytes_ext(mc, nullptr, tc, world, layout, bytes_out);
+}
+int32_t dtx_plan_device_bytes_ext(const dtx_model_cfg* mc, const dtx_model_ext* ext, const dtx_train_cfg* tc, int32_t world,
+                                  int32_t layout, int64_t* bytes_out) {
   if (!mc || !tc || !bytes_out || world < 1) {
     g_error = "plan_device_bytes: null argument or world < 1";
     return DTX_ERR_INVALID;
@@ -2024,9 +2147,10 @@ int32_t dtx_plan_device_bytes(const dtx_model_cfg* mc, const dtx_train_cfg* tc, 
     g_error = "plan_device_bytes: layout must be 1 (keep all activations) or 2 (recompute per layer)";
     return DTX_ERR_INVALID;
   }
-  const int rc = check_cfg(mc, tc);
+  int rc = check_cfg(mc, tc);
+  if (rc == DTX_OK) rc = check_ext(ext);
   if (rc) return rc;
-  *bytes_out = planned_bytes(mc, tc, world, 132, layout);  // split-K buffers sized for the 132 SMs of an H100 SXM
+  *bytes_out = planned_bytes(mc, ext, tc, world, 132, layout);  // split-K buffers sized for the 132 SMs of an H100 SXM
   return DTX_OK;
 }
 int64_t dtx_launch_count(const dtx_trainer* t) { return t ? t->launches : 0; }

@@ -24,6 +24,8 @@ EPI_BF16, EPI_F32, EPI_BF16_ADD, EPI_ROPE, EPI_SWIGLU_FWD, EPI_SWIGLU_BWD = 0, 1
 STEP_FORCE = 1
 # activation layouts (dtx_train_cfg.recompute): automatic, every layer keeps its activations, one shared set recomputed per layer
 RECOMPUTE = {"auto": 0, "keep": 1, "layer": 2}
+# rotary inverse-frequency types (dtx_model_ext.rope_type), by HF `rope_type` name
+ROPE_TYPES = {"default": 0, "linear": 1, "llama3": 2}
 
 
 class DtxError(RuntimeError):
@@ -38,6 +40,11 @@ class ModelCfg(C.Structure):
                 ("rope_theta", C.c_float), ("max_seq", C.c_int32), ("sliding_window", C.c_int32)]
 
 
+class ModelExt(C.Structure):
+    _fields_ = [("qkv_bias", C.c_int32), ("rope_type", C.c_int32), ("rope_factor", C.c_float),
+                ("rope_low_freq_factor", C.c_float), ("rope_high_freq_factor", C.c_float), ("rope_original_max_pos", C.c_int32)]
+
+
 class TrainCfg(C.Structure):
     _fields_ = [("lora_r", C.c_int32), ("lora_alpha", C.c_float), ("lora_dropout", C.c_float),
                 ("target_mask", C.c_uint32), ("lr", C.c_float), ("weight_decay", C.c_float), ("beta1", C.c_float),
@@ -49,7 +56,8 @@ class TrainCfg(C.Structure):
 
 # every symbol include/dtxtune.h declares (tests/test_abi.py checks the .so exports all of them)
 ABI_SYMBOLS = [
-    "dtx_abi_version", "dtx_last_global_error", "dtx_last_error", "dtx_trainer_create", "dtx_trainer_destroy",
+    "dtx_abi_version", "dtx_last_global_error", "dtx_last_error", "dtx_trainer_create", "dtx_trainer_create_ext",
+    "dtx_rope_inv_freq", "dtx_plan_device_bytes_ext", "dtx_gemm_bias", "dtx_bias_grad", "dtx_trainer_destroy",
     "dtx_get_nccl_unique_id", "dtx_load_tensor", "dtx_init_random_weights", "dtx_init_lora", "dtx_quantize_base", "dtx_step",
     "dtx_step_device", "dtx_eval_loss", "dtx_allreduce_host", "dtx_export_adapter", "dtx_export_adapter_grad", "dtx_export_weight", "dtx_num_trainable", "dtx_launch_count",
     "dtx_recompute", "dtx_device_bytes", "dtx_plan_device_bytes",
@@ -78,6 +86,13 @@ def load() -> C.CDLL:
     lib.dtx_last_error.restype = C.c_char_p
     lib.dtx_last_error.argtypes = [vp]
     lib.dtx_trainer_create.argtypes = [C.POINTER(ModelCfg), C.POINTER(TrainCfg), i32, i32, i32, vp, C.POINTER(vp)]
+    lib.dtx_trainer_create_ext.argtypes = [C.POINTER(ModelCfg), C.POINTER(ModelExt), C.POINTER(TrainCfg), i32, i32, i32, vp,
+                                           C.POINTER(vp)]
+    lib.dtx_rope_inv_freq.argtypes = [C.POINTER(ModelCfg), C.POINTER(ModelExt), vp]
+    lib.dtx_plan_device_bytes_ext.argtypes = [C.POINTER(ModelCfg), C.POINTER(ModelExt), C.POINTER(TrainCfg), i32, i32, C.POINTER(i64)]
+    lib.dtx_gemm_bias.argtypes = [vp, i64, vp, i64, i32, vp, i64, vp, i64, i32, vp, i64, vp, i64, vp, i32, i32, vp, i32, i32, i32,
+                                  i32, vp, vp]
+    lib.dtx_bias_grad.argtypes = [vp, i64, i32, i32, vp, i32, vp]
     lib.dtx_trainer_destroy.argtypes = [vp]
     lib.dtx_trainer_destroy.restype = None
     lib.dtx_get_nccl_unique_id.argtypes = [vp]
@@ -180,9 +195,18 @@ def plan_device_bytes(model: "ModelConfig", train: "TrainConfig", world: int = 1
     """Bytes of device memory a trainer for this configuration allocates per rank with activation layout "keep" or "layer"
     (host arithmetic inside the library, no GPU needed)."""
     code = RECOMPUTE[layout] if isinstance(layout, str) else int(layout)
-    mc, tc, out = model.to_c(), train.to_c(), C.c_int64()
-    check(load().dtx_plan_device_bytes(C.byref(mc), C.byref(tc), world, code, C.byref(out)))
+    mc, ext, tc, out = model.to_c(), model.ext_to_c(), train.to_c(), C.c_int64()
+    check(load().dtx_plan_device_bytes_ext(C.byref(mc), C.byref(ext), C.byref(tc), world, code, C.byref(out)))
     return int(out.value)
+
+
+def rope_inv_freq(model: "ModelConfig") -> np.ndarray:
+    """The fp32 inverse frequencies the trainer builds its rotary table from (head_dim / 2 values; host arithmetic inside the
+    library, no GPU needed)."""
+    mc, ext = model.to_c(), model.ext_to_c()
+    out = np.zeros(model.head_dim // 2, np.float32)
+    check(load().dtx_rope_inv_freq(C.byref(mc), C.byref(ext), out.ctypes.data_as(C.c_void_p)))
+    return out
 
 
 def lr_lambda(sched: str, step: int, warmup: int, total: int) -> float:
@@ -203,6 +227,10 @@ class ModelConfig:
     rope_theta: float = 10000.0
     max_seq: int = 4096
     sliding_window: int = 0            # Mistral config.json `sliding_window`; 0 = none
+    qkv_bias: bool = False             # q_proj / k_proj / v_proj carry a bias (Qwen2)
+    # HF config.json `rope_scaling` / `rope_parameters`: {"rope_type" (or the older "type"): "linear" | "llama3", "factor", ...};
+    # None = the plain theta table
+    rope_scaling: Optional[dict] = None
 
     @staticmethod
     def llama2_7b() -> "ModelConfig":
@@ -211,6 +239,16 @@ class ModelConfig:
     def to_c(self) -> ModelCfg:
         return ModelCfg(self.vocab, self.hidden, self.n_layers, self.n_heads, self.n_kv_heads or self.n_heads,
                         self.head_dim, self.ffn, self.rms_eps, self.rope_theta, self.max_seq, int(self.sliding_window or 0))
+
+    def ext_to_c(self) -> ModelExt:
+        rs = self.rope_scaling or {}
+        kind = rs.get("rope_type", rs.get("type", "default"))
+        if kind not in ROPE_TYPES:
+            raise DtxError(-1, f"rope_type {kind!r}: only {', '.join(ROPE_TYPES)} are implemented natively")
+        if kind == "default":
+            return ModelExt(int(bool(self.qkv_bias)), 0, 0.0, 0.0, 0.0, 0)
+        return ModelExt(int(bool(self.qkv_bias)), ROPE_TYPES[kind], float(rs["factor"]), float(rs.get("low_freq_factor", 0.0)),
+                        float(rs.get("high_freq_factor", 0.0)), int(rs.get("original_max_position_embeddings", 0)))
 
 
 @dataclass
@@ -260,11 +298,11 @@ class Trainer:
         self.lib = load()
         self.model, self.train = model, train
         self._h = C.c_void_p()
-        mc, tc = model.to_c(), train.to_c()
+        mc, ext, tc = model.to_c(), model.ext_to_c(), train.to_c()
         if world > 1:
             preload_nccl()
         idbuf = C.create_string_buffer(nccl_id, 128) if nccl_id is not None else None
-        check(self.lib.dtx_trainer_create(C.byref(mc), C.byref(tc), device, rank, world, idbuf, C.byref(self._h)))
+        check(self.lib.dtx_trainer_create_ext(C.byref(mc), C.byref(ext), C.byref(tc), device, rank, world, idbuf, C.byref(self._h)))
 
     def close(self) -> None:
         if self._h:
@@ -389,6 +427,10 @@ class Trainer:
             yield p + "self_attn.q_proj.weight", (d, d)
             yield p + "self_attn.k_proj.weight", (dkv, d)
             yield p + "self_attn.v_proj.weight", (dkv, d)
+            if m.qkv_bias:
+                yield p + "self_attn.q_proj.bias", (d,)
+                yield p + "self_attn.k_proj.bias", (dkv,)
+                yield p + "self_attn.v_proj.bias", (dkv,)
             yield p + "self_attn.o_proj.weight", (d, d)
             yield p + "mlp.gate_proj.weight", (F, d)
             yield p + "mlp.up_proj.weight", (F, d)

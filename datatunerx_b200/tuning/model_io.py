@@ -1,6 +1,7 @@
 """Model / adapter file IO of the worker, numpy only (no torch, no safetensors package needed at run time).
 
-  * load_model_config  : HF config.json -> ModelConfig  (AutoConfig.from_pretrained, cmd/tuning/train.py:221)
+  * load_model_config  : HF config.json -> ModelConfig  (AutoConfig.from_pretrained, cmd/tuning/train.py:221): Llama-2,
+                         Llama-3.x (linear / llama3 rope scaling), Mistral, Qwen2 / Qwen2.5 (q/k/v biases)
   * iter_safetensors   : stream tensors of *.safetensors shards (AutoModelForCausalLM.from_pretrained, train.py:236-242);
                          iter_torch_bin does the same for pytorch_model*.bin shards
   * save_peft_adapter  : adapter_config.json + adapter_model.safetensors (+ adapter_model.bin when torch is importable)
@@ -22,16 +23,42 @@ from ..lib import ModelConfig
 _ST_DTYPES = {"F32": (np.float32, 4, False), "F16": (np.float16, 2, False), "BF16": (np.uint16, 2, True)}
 
 
-def load_model_config(model_dir: str) -> ModelConfig:
+# HF rope types whose inverse frequencies the library builds (dtx_model_ext.rope_type); yarn, dynamic, longrope... are refused
+_ROPE_TYPES = ("default", "linear", "llama3")
+
+
+def load_model_config(model_dir: str, full_finetune: bool = False) -> ModelConfig:
+    """HF config.json -> ModelConfig for the decoders the library trains: Llama-2 / Llama-3.x (`rope_scaling` of type linear or
+    llama3), Mistral and Qwen2 / Qwen2.5 (q/k/v biases).  Anything that would train a different model than HF's raises ValueError."""
     cfg = json.load(open(os.path.join(model_dir, "config.json")))
     arch = (cfg.get("architectures") or ["LlamaForCausalLM"])[0]
-    if "Llama" not in arch and "Mistral" not in arch:
-        raise ValueError(f"{arch}: only Llama-family decoders are implemented natively")
+    qwen2 = arch == "Qwen2ForCausalLM"
+    if "Llama" not in arch and "Mistral" not in arch and not qwen2:
+        raise ValueError(f"{arch}: only Llama-family and Qwen2 decoders are implemented natively")
+    if cfg.get("attention_bias") or cfg.get("mlp_bias"):
+        raise ValueError(f"{arch}: attention_bias / mlp_bias are not implemented natively")
+    # transformers 5 names the dict `rope_parameters` (it then also carries rope_theta); older configs `rope_scaling`
+    rs = cfg.get("rope_scaling") or cfg.get("rope_parameters") or None
+    rope_theta = cfg.get("rope_theta", (rs or {}).get("rope_theta", 10000.0))
+    if rs is not None:
+        kind = rs.get("rope_type", rs.get("type", "default"))
+        if kind not in _ROPE_TYPES:
+            raise ValueError(f"rope_scaling type {kind!r} is not implemented natively (supported: {', '.join(_ROPE_TYPES)})")
+        rs = None if kind == "default" else dict(rs)
+    window = int(cfg.get("sliding_window") or 0)
+    if qwen2:
+        # Qwen2.5 ships sliding_window = 131072 with use_sliding_window = false: HF then attends over the whole causal window
+        if cfg.get("use_sliding_window"):
+            raise ValueError("Qwen2 use_sliding_window (per-layer sliding windows) is not implemented natively")
+        window = 0
+        if full_finetune and cfg.get("tie_word_embeddings"):
+            raise ValueError("full-parameter SFT of a Qwen2 checkpoint with tie_word_embeddings would train the embedding and "
+                             "lm_head as two tensors, unlike HF; use LoRA")
     heads = cfg["num_attention_heads"]
     return ModelConfig(vocab=cfg["vocab_size"], hidden=cfg["hidden_size"], n_layers=cfg["num_hidden_layers"], n_heads=heads,
                        n_kv_heads=cfg.get("num_key_value_heads", heads), head_dim=cfg.get("head_dim") or cfg["hidden_size"] // heads,
-                       ffn=cfg["intermediate_size"], rms_eps=cfg.get("rms_norm_eps", 1e-5), rope_theta=cfg.get("rope_theta", 10000.0),
-                       max_seq=cfg.get("max_position_embeddings", 4096), sliding_window=int(cfg.get("sliding_window") or 0))
+                       ffn=cfg["intermediate_size"], rms_eps=cfg.get("rms_norm_eps", 1e-5), rope_theta=rope_theta,
+                       max_seq=cfg.get("max_position_embeddings", 4096), sliding_window=window, qkv_bias=qwen2, rope_scaling=rs)
 
 
 def check_attention_window(model_dir: str, seq_len: int) -> None:

@@ -83,14 +83,14 @@ def run_rank(a: TrainArgs, rank: int, world: int, nccl_id: Optional[bytes], toke
         raise RuntimeError(f"{len(dataset)} training examples cannot be split over {world} workers")
     eval_set = dataset if a.evaluation_path else None  # the reference re-reads the TRAIN file for eval (train.py:347)
 
-    mc = model_io.load_model_config(a.model_name_or_path)
+    # The reference parses --finetuning_type and then wraps LoRA regardless (cmd/tuning/train.py:266-280): a drop-in must do the
+    # same.  Full-parameter SFT (BASELINE.json configs[3]) is an explicit opt-in on top: DTX_HONOR_FINETUNING_TYPE=1.
+    full = a.finetuning_type == "full" and os.environ.get("DTX_HONOR_FINETUNING_TYPE") == "1"
+    mc = model_io.load_model_config(a.model_name_or_path, full_finetune=full)
     seq_len = D.static_seq_len(cutoff_len)
     model_io.check_attention_window(a.model_name_or_path, seq_len)
     B, GA = a.per_device_train_batch_size, max(1, a.gradient_accumulation_steps)
     total = total_optimizer_steps(len(dataset), world, B, GA, a.num_train_epochs, a.max_steps)
-    # The reference parses --finetuning_type and then wraps LoRA regardless (cmd/tuning/train.py:266-280): a drop-in must do the
-    # same.  Full-parameter SFT (BASELINE.json configs[3]) is an explicit opt-in on top: DTX_HONOR_FINETUNING_TYPE=1.
-    full = a.finetuning_type == "full" and os.environ.get("DTX_HONOR_FINETUNING_TYPE") == "1"
     if a.finetuning_type != "lora" and not full and rank == 0:
         print(f"[dtx] --finetuning_type {a.finetuning_type} is ignored like in the reference worker (LoRA is always applied); "
               "set DTX_HONOR_FINETUNING_TYPE=1 for native full-parameter SFT", flush=True)

@@ -87,6 +87,19 @@ typedef struct {
   int32_t recompute;
 } dtx_train_cfg;
 
+/* Model-family extensions of dtx_model_cfg (Llama-3.1 / 3.2 scaled rotary tables, Qwen2 q/k/v projection biases).  A NULL
+ * or all-zero dtx_model_ext is the plain Llama-2 / Mistral model: no bias, rotary inverse frequencies theta^(-2i/D). */
+#define DTX_ROPE_DEFAULT 0   /* inv_freq = theta^(-2i/D) */
+#define DTX_ROPE_LINEAR  1   /* inv_freq / factor (HF rope_type "linear") */
+#define DTX_ROPE_LLAMA3  2   /* HF _compute_llama3_parameters (Llama-3.1 / 3.2): high frequencies kept, low ones / factor,
+                                smooth interpolation between; attention scaling 1 */
+typedef struct {
+  int32_t qkv_bias;                 /* 1: q_proj / k_proj / v_proj carry a bias (Qwen2) */
+  int32_t rope_type;                /* DTX_ROPE_* */
+  float rope_factor, rope_low_freq_factor, rope_high_freq_factor;  /* factor: linear and llama3; the two others: llama3 */
+  int32_t rope_original_max_pos;    /* llama3: original_max_position_embeddings */
+} dtx_model_ext;
+
 typedef struct dtx_trainer dtx_trainer;
 
 /* ---- library ---- */
@@ -99,6 +112,14 @@ DTX_API const char* dtx_last_error(const dtx_trainer* t);
 /* nccl_unique_id: 128 bytes from dtx_get_nccl_unique_id on rank 0 (world > 1), else NULL. */
 DTX_API int32_t dtx_trainer_create(const dtx_model_cfg* model, const dtx_train_cfg* train, int32_t device, int32_t rank,
                            int32_t world, const void* nccl_unique_id, dtx_trainer** out);
+/* The same for a model with family extensions (ext may be NULL: dtx_trainer_create).  An unknown rope_type, a factor <= 0, or
+ * for llama3 low_freq_factor >= high_freq_factor or original_max_pos <= 0 return DTX_ERR_INVALID before any device work.
+ * With qkv_bias, "model.layers.N.self_attn.{q,k,v}_proj.bias" must be loaded before a step; full-parameter SFT trains them
+ * without weight decay (HF get_decay_parameter_names), LoRA keeps them frozen (peft bias="none"). */
+DTX_API int32_t dtx_trainer_create_ext(const dtx_model_cfg* model, const dtx_model_ext* ext, const dtx_train_cfg* train,
+                                       int32_t device, int32_t rank, int32_t world, const void* nccl_unique_id, dtx_trainer** out);
+/* host arithmetic, no device: the fp32 inverse frequencies the rotary table is built from (head_dim / 2 values) */
+DTX_API int32_t dtx_rope_inv_freq(const dtx_model_cfg* model, const dtx_model_ext* ext, float* out);
 DTX_API void dtx_trainer_destroy(dtx_trainer* t);
 DTX_API int32_t dtx_get_nccl_unique_id(void* out128);
 
@@ -168,6 +189,10 @@ DTX_API int64_t dtx_device_bytes(const dtx_trainer* t);
  * device).  The small split-K partial buffers of the adapter gradients are sized for the 132 SMs of an H100 SXM. */
 DTX_API int32_t dtx_plan_device_bytes(const dtx_model_cfg* model, const dtx_train_cfg* train, int32_t world, int32_t layout,
                                       int64_t* bytes_out);
+/* the same for a model with family extensions (ext may be NULL): counts the q|k|v bias vectors and, under full-parameter SFT,
+ * their gradients and optimizer shards */
+DTX_API int32_t dtx_plan_device_bytes_ext(const dtx_model_cfg* model, const dtx_model_ext* ext, const dtx_train_cfg* train,
+                                          int32_t world, int32_t layout, int64_t* bytes_out);
 /* kernels launched by this trainer since creation (bench.py's gpu_launches) */
 DTX_API int64_t dtx_launch_count(const dtx_trainer* t);
 /* device time of the most recent dtx_step in ms (CUDA events on the trainer's stream) */
@@ -224,6 +249,17 @@ DTX_API int32_t dtx_gemm_fused(const void* A, int64_t lda, const void* B, int64_
                        int64_t lda2, const void* B2, int64_t ldb2, int32_t K2, void* C, int64_t ldc, void* aux, int64_t ld_aux,
                        const void* rope_cs, int32_t rope_S, int32_t rope_cols, int32_t M, int32_t N, int32_t K,
                        int32_t epilogue, void* stream);
+/* dtx_gemm_fused's arguments plus bias: a device bf16 [N] vector added to the fp32 accumulator before the rounding (epilogue 0,
+ * EPI_BF16) or before the rotary (epilogue 3, EPI_ROPE) - HF's q = x W^T + b, then RoPE.  Other epilogues: DTX_ERR_INVALID.
+ * rope_pos (epilogue 3, optional device int32 [M]): position of every row inside its sequence (packed ragged batches); NULL:
+ * row % rope_S.  Epilogue 0 takes the tile width from the "gemm_pair_kernel" switch like dtx_gemm_bf16 with block_n = 0. */
+DTX_API int32_t dtx_gemm_bias(const void* A, int64_t lda, const void* B, int64_t ldb, int32_t b_mn_major, const void* A2,
+                              int64_t lda2, const void* B2, int64_t ldb2, int32_t K2, void* C, int64_t ldc, void* aux, int64_t ld_aux,
+                              const void* rope_cs, int32_t rope_S, int32_t rope_cols, const void* rope_pos, int32_t M, int32_t N,
+                              int32_t K, int32_t epilogue, const void* bias, void* stream);
+/* bias gradient: db[n] (+)= sum_m dy[m, n] over a bf16 [M, n] matrix with row stride ld (fp32, fixed summation order);
+ * accumulate = 0 overwrites db (bf16 [n]) */
+DTX_API int32_t dtx_bias_grad(const void* dy, int64_t ld, int32_t M, int32_t n, void* db, int32_t accumulate, void* stream);
 DTX_API int32_t dtx_embedding_fwd(const void* ids, const void* table, void* out, int32_t M, int32_t d, int32_t vocab, void* stream);
 DTX_API int32_t dtx_rmsnorm_fwd(const void* x, const void* w, void* y, void* rstd, int32_t M, int32_t d, float eps, void* stream);
 DTX_API int32_t dtx_rmsnorm_bwd(const void* dy, const void* x, const void* w, const void* rstd, const void* dres, void* dx,

@@ -1,0 +1,137 @@
+"""Throughput of the model families beyond Llama-2 on one GPU, and the cost of the q|k|v bias in the GEMM epilogue.
+
+  * Llama-3.1-8B shape (vocab 128 256, GQA 32 / 8, FFN 14 336, llama3 rope scaling) and Qwen2.5-7B shape (q/k/v biases, GQA 28 / 4,
+    FFN 18 944, vocab 152 064), random-init weights, LoRA r=16 on q_proj,v_proj, micro-batch 4 x 2048 - the headline bench.py
+    workload on the checkpoints people fine-tune today.  Per config: tokens/s of `--runs` timed windows of `--steps` optimizer
+    steps (median and range), the activation layout automatic mode chose, the planned and the held device bytes.
+  * The Qwen2.5-7B q|k|v GEMM (M 8192 x N 4608 x K 3584, fused RoPE epilogue) with and without the bias, alternated in one
+    process, timed with CUDA events.
+
+The card's name and power limit are read in the same run and printed with the numbers.  Prints one JSON document; --out also
+writes it to a file.
+"""
+from __future__ import annotations
+
+import argparse
+import ctypes as C
+import json
+import os
+import statistics
+import subprocess
+import sys
+import time
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+if ROOT not in sys.path:
+    sys.path.insert(0, ROOT)
+
+from datatunerx_b200 import lib as L  # noqa: E402
+from datatunerx_b200.tuning.synthetic import synthetic_batch  # noqa: E402
+
+CONFIGS = {
+    "llama3.1-8b": L.ModelConfig(vocab=128256, hidden=4096, n_layers=32, n_heads=32, n_kv_heads=8, ffn=14336, rope_theta=500000.0,
+                                 max_seq=131072,
+                                 rope_scaling={"rope_type": "llama3", "factor": 8.0, "low_freq_factor": 1.0, "high_freq_factor": 4.0,
+                                               "original_max_position_embeddings": 8192}),
+    "qwen2.5-7b": L.ModelConfig(vocab=152064, hidden=3584, n_layers=28, n_heads=28, n_kv_heads=4, ffn=18944, rope_theta=1000000.0,
+                                rms_eps=1e-6, max_seq=32768, qkv_bias=True),
+}
+
+
+def card() -> dict:
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
+    name, _, power = q.stdout.strip().splitlines()[0].partition(",")
+    return {"name": name.strip(), "power_limit": power.strip()}
+
+
+def train_throughput(name: str, mc: L.ModelConfig, B: int, S: int, steps: int, warmup: int, runs: int) -> dict:
+    tc = L.TrainConfig(micro_batch=B, seq_len=S, total_steps=10 ** 6, lora_r=16, lora_alpha=32.0, lora_dropout=0.0, lr=1e-4)
+    planned = {k: L.plan_device_bytes(mc, tc, 1, k) for k in ("keep", "layer")}
+    tr = L.Trainer(mc, tc)
+    tr.init_random_weights(1234)
+    tr.init_lora(4321)
+    batches = [synthetic_batch(s, 0, B, S, mc.vocab) for s in range(4)]
+    for s in range(warmup):
+        tr.step(*batches[s % 4])
+    rates, losses = [], []
+    for _ in range(runs):
+        t0 = time.perf_counter()
+        for s in range(steps):  # dtx_step returns after the step has finished on the device
+            loss, _, _, _ = tr.step(*batches[s % 4])
+        rates.append(B * S * steps / (time.perf_counter() - t0))
+        losses.append(loss)
+    out = {"config": name, "tokens_per_s_median": statistics.median(rates), "tokens_per_s_range": [min(rates), max(rates)],
+           "layout": tr.recompute, "planned_bytes": planned, "held_bytes": tr.device_bytes, "last_loss": losses[-1]}
+    tr.close()
+    return out
+
+
+def bias_gemm_cost(iters: int, rounds: int) -> dict:
+    import torch
+    M, N, K, H, Hkv, D = 8192, 4608, 3584, 28, 4, 128
+    lib = L.load()
+    g = torch.Generator().manual_seed(0)
+    A = (torch.randn(M, K, generator=g) * 0.5).to(torch.bfloat16).cuda()
+    Bw = (torch.randn(N, K, generator=g) * 0.02).to(torch.bfloat16).cuda()
+    bias = (torch.randn(N, generator=g) * 0.1).to(torch.bfloat16).cuda()
+    Cm = torch.empty(M, N, dtype=torch.bfloat16, device="cuda")
+    cs = torch.empty(S_ROPE, D // 2, 2, dtype=torch.float32, device="cuda")
+    stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+    L.check(lib.dtx_rope_table(C.c_void_p(cs.data_ptr()), S_ROPE, D, 1000000.0, stream))
+    P = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None  # noqa: E731
+
+    def launch(with_bias: bool):
+        L.check(lib.dtx_gemm_bias(P(A), K, P(Bw), K, 0, None, 0, None, 0, 0, P(Cm), N, None, 0, P(cs), S_ROPE, (H + Hkv) * D, None,
+                                  M, N, K, L.EPI_ROPE, P(bias), stream) if with_bias else
+                lib.dtx_gemm_fused(P(A), K, P(Bw), K, 0, None, 0, None, 0, 0, P(Cm), N, None, 0, P(cs), S_ROPE, (H + Hkv) * D,
+                                   M, N, K, L.EPI_ROPE, stream))
+
+    for wb in (False, True):
+        for _ in range(10):
+            launch(wb)
+    times = {False: [], True: []}
+    for _ in range(rounds):
+        for wb in (False, True):
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            for _ in range(iters):
+                launch(wb)
+            e1.record()
+            torch.cuda.synchronize()
+            times[wb].append(e0.elapsed_time(e1) / iters)
+    flop = 2.0 * M * N * K
+    res = {}
+    for wb, key in ((False, "no_bias"), (True, "bias")):
+        ms = statistics.median(times[wb])
+        res[key] = {"ms_median": ms, "ms_range": [min(times[wb]), max(times[wb])], "tflops": flop / ms / 1e9}
+    res["shape"] = [M, N, K]
+    return res
+
+
+S_ROPE = 2048
+
+
+def main() -> None:
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=8)
+    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--runs", type=int, default=4)
+    ap.add_argument("--batch", type=int, default=4)
+    ap.add_argument("--seq", type=int, default=2048)
+    ap.add_argument("--configs", default=",".join(CONFIGS))
+    ap.add_argument("--out", default=None)
+    a = ap.parse_args()
+    res = {"card": card(), "lora": "r=16 on q_proj,v_proj", "micro_batch": a.batch, "seq_len": a.seq, "runs": []}
+    for name in a.configs.split(","):
+        res["runs"].append(train_throughput(name, CONFIGS[name], a.batch, a.seq, a.steps, a.warmup, a.runs))
+        print(json.dumps(res["runs"][-1]), flush=True)
+    res["qkv_gemm_bias_cost"] = bias_gemm_cost(iters=50, rounds=6)
+    res["card_after"] = card()
+    print(json.dumps(res, indent=1))
+    if a.out:
+        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
+        json.dump(res, open(a.out, "w"), indent=1)
+
+
+if __name__ == "__main__":
+    main()
