@@ -61,6 +61,37 @@ int32_t dtx_bias_grad(const void* dy, int64_t ld, int32_t M, int32_t n, void* db
   return rc(bias_grad(static_cast<const bf16*>(dy), ld, M, n, static_cast<bf16*>(db), accumulate, S(stream)));
 }
 
+int32_t dtx_gemm_qk_norm(const void* A, int64_t lda, const void* B, int64_t ldb, int32_t b_mn, const void* A2, int64_t lda2,
+                         const void* B2, int64_t ldb2, int32_t K2, void* C, int64_t ldc, void* aux, int64_t ld_aux, const void* rope_cs,
+                         int32_t rope_S, int32_t rope_cols, const void* rope_pos, int32_t M, int32_t N, int32_t K, int32_t q_cols,
+                         const void* wq, const void* wk, float eps, void* stream) {
+  if (!wq || !wk) return DTX_ERR_INVALID;
+  GemmArgs g;
+  g.A = static_cast<const bf16*>(A); g.lda = lda;
+  g.B = static_cast<const bf16*>(B); g.ldb = ldb; g.b_mn_major = b_mn;
+  g.A2 = static_cast<const bf16*>(A2); g.lda2 = lda2; g.B2 = static_cast<const bf16*>(B2); g.ldb2 = ldb2; g.K2 = K2;
+  g.C = C; g.ldc = ldc; g.aux = aux; g.ld_aux = ld_aux;
+  g.rope_cs = static_cast<const float2*>(rope_cs); g.rope_S = rope_S; g.rope_cols = rope_cols;
+  g.rope_pos = static_cast<const int32_t*>(rope_pos);
+  g.M = M; g.N = N; g.K = K; g.epilogue = EPI_ROPE;
+  g.qk_wq = static_cast<const bf16*>(wq); g.qk_wk = static_cast<const bf16*>(wk); g.qk_q_cols = q_cols; g.qk_eps = eps;
+  return rc(gemm_bf16(g, S(stream)));
+}
+
+int32_t dtx_qk_norm_fwd(void* qkv, int64_t ld, int32_t M, int32_t q_cols, int32_t n_cols, const void* wq, const void* wk, float eps,
+                        void* pre, int64_t ld_pre, void* stream) {
+  return rc(qk_norm_fwd(static_cast<bf16*>(qkv), ld, M, q_cols, n_cols, static_cast<const bf16*>(wq), static_cast<const bf16*>(wk), eps,
+                        static_cast<bf16*>(pre), ld_pre, S(stream)));
+}
+
+int32_t dtx_qk_norm_bwd(void* dy, int64_t ld, const void* x, int64_t ldx, int32_t M, int32_t q_cols, int32_t n_cols, const void* wq,
+                        const void* wk, float eps, void* dw, void* scratch, int32_t nblk, int32_t accumulate, void* stream) {
+  if (dw && (nblk < 1 || nblk > QKN_MAX_BLOCKS)) return DTX_ERR_INVALID;
+  return rc(qk_norm_bwd(static_cast<bf16*>(dy), ld, static_cast<const bf16*>(x), ldx, M, q_cols, n_cols, static_cast<const bf16*>(wq),
+                        static_cast<const bf16*>(wk), eps, static_cast<bf16*>(dw), static_cast<float*>(scratch), nblk, accumulate,
+                        S(stream)));
+}
+
 int32_t dtx_set_option(const char* name, int32_t value) {
   if (!name) return DTX_ERR_INVALID;
   if (strcmp(name, "gemm_pair_kernel") == 0) {

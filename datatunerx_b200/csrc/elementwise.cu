@@ -777,6 +777,101 @@ __global__ void __launch_bounds__(256) bias_grad_kernel(const bf16* __restrict__
     db[c + 1] = __float2bfloat16_rn(y);
   }
 }
+// ------------------------------------------------------------------------------------------
+// Qwen3 q/k RMSNorm over each 128-value head of the q|k columns of packed qkv (columns < n_cols; w = wq below q_cols, wk
+// beyond).  One warp per (row, head), four consecutive values per lane, warp_sum (fixed order) for the two reductions.
+// ------------------------------------------------------------------------------------------
+__device__ __forceinline__ void ld_bf16x4(const bf16* p, float (&f)[4]) {
+  const uint2 u = *reinterpret_cast<const uint2*>(p);
+  const float2 a = unpack_bf16x2(u.x), b = unpack_bf16x2(u.y);
+  f[0] = a.x; f[1] = a.y; f[2] = b.x; f[3] = b.y;
+}
+__device__ __forceinline__ void st_bf16x4(bf16* p, const float (&f)[4]) {
+  *reinterpret_cast<uint2*>(p) = make_uint2(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]));
+}
+// forward, in place: x_pre (aux) = x, x = w * (x * rsqrt(mean(x^2) + eps)) - the unfused path's epilogue (fp32, like EPI_ROPE's)
+__global__ void __launch_bounds__(256) qk_norm_fwd_kernel(bf16* __restrict__ qkv, long long ld, int M, int q_cols, int n_cols,
+                                                          const bf16* __restrict__ wq, const bf16* __restrict__ wk, float eps,
+                                                          bf16* __restrict__ pre, long long ld_pre) {
+  const int nh = n_cols >> 7, lane = threadIdx.x & 31;
+  const long long items = static_cast<long long>(M) * nh;
+  for (long long it = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5; it < items;
+       it += (static_cast<long long>(gridDim.x) * blockDim.x) >> 5) {
+    const long long m = it / nh;
+    const int c = static_cast<int>(it % nh) * 128 + lane * 4;
+    bf16* xp = qkv + m * ld + c;
+    float x[4], w[4];
+    ld_bf16x4(xp, x);
+    ld_bf16x4((c < q_cols ? wq : wk) + (c & 127), w);
+    st_bf16x4(pre + m * ld_pre + c, x);
+    const float r = rsqrtf(warp_sum(x[0] * x[0] + x[1] * x[1] + x[2] * x[2] + x[3] * x[3]) * (1.f / 128.f) + eps);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) x[j] = x[j] * r * w[j];
+    st_bf16x4(xp, x);
+  }
+}
+// backward, in place on dy: x = the saved pre-norm values, rstd recomputed, xh = x * rstd, g = w * dy,
+// dx = rstd * (g - xh * mean(g * xh)).  part (optional): block b's fp32 sums of dy * xh over its items, [b][0..127] q heads,
+// [b][128..255] k heads (the items of a block and their order depend on the grid only: fixed summation order)
+__global__ void __launch_bounds__(256) qk_norm_bwd_kernel(bf16* __restrict__ dy, long long ld, const bf16* __restrict__ xs,
+                                                          long long ldx, int M, int q_cols, int n_cols, const bf16* __restrict__ wq,
+                                                          const bf16* __restrict__ wk, float eps, float* __restrict__ part) {
+  __shared__ float sh[8][256];
+  const int nh = n_cols >> 7, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const long long items = static_cast<long long>(M) * nh;
+  float aq[4] = {0.f, 0.f, 0.f, 0.f}, ak[4] = {0.f, 0.f, 0.f, 0.f};
+  for (long long it = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5; it < items;
+       it += (static_cast<long long>(gridDim.x) * blockDim.x) >> 5) {
+    const long long m = it / nh;
+    const int c = static_cast<int>(it % nh) * 128 + lane * 4;
+    bf16* gp = dy + m * ld + c;
+    const bool is_q = c < q_cols;
+    float x[4], g[4], w[4];
+    ld_bf16x4(xs + m * ldx + c, x);
+    ld_bf16x4(gp, g);
+    ld_bf16x4((is_q ? wq : wk) + (c & 127), w);
+    const float r = rsqrtf(warp_sum(x[0] * x[0] + x[1] * x[1] + x[2] * x[2] + x[3] * x[3]) * (1.f / 128.f) + eps);
+    float dot = 0.f;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float xh = x[j] * r;
+      if (part) {
+        if (is_q) aq[j] += g[j] * xh;
+        else ak[j] += g[j] * xh;
+      }
+      x[j] = xh;
+      g[j] *= w[j];
+      dot += g[j] * xh;
+    }
+    const float mean = warp_sum(dot) * (1.f / 128.f);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) g[j] = r * (g[j] - x[j] * mean);
+    st_bf16x4(gp, g);
+  }
+  if (!part) return;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    sh[warp][lane * 4 + j] = aq[j];
+    sh[warp][128 + lane * 4 + j] = ak[j];
+  }
+  __syncthreads();
+  const int c = threadIdx.x;
+  part[static_cast<size_t>(blockIdx.x) * 256 + c] =
+      ((sh[0][c] + sh[1][c]) + (sh[2][c] + sh[3][c])) + ((sh[4][c] + sh[5][c]) + (sh[6][c] + sh[7][c]));
+}
+// dw[c] (+)= sum_b part[b][c]: 32 columns x 8 lanes per block, lane r adds partials r, r + 8, ... then a fixed tree
+__global__ void __launch_bounds__(256) qk_norm_dw_kernel(const float* __restrict__ part, int nblk, bf16* __restrict__ dw, int accumulate) {
+  __shared__ float sh[8][32];
+  const int cl = threadIdx.x & 31, lane_r = threadIdx.x >> 5, c = blockIdx.x * 32 + cl;
+  float acc = 0.f;
+  for (int b = lane_r; b < nblk; b += 8) acc += part[static_cast<size_t>(b) * 256 + c];
+  sh[lane_r][cl] = acc;
+  __syncthreads();
+  if (lane_r) return;
+  float v = ((sh[0][cl] + sh[1][cl]) + (sh[2][cl] + sh[3][cl])) + ((sh[4][cl] + sh[5][cl]) + (sh[6][cl] + sh[7][cl]));
+  if (accumulate) v += __bfloat162float(dw[c]);
+  dw[c] = __float2bfloat16_rn(v);
+}
 __global__ void embedding_bwd_kernel(const int32_t* __restrict__ ids, const bf16* __restrict__ dx, float* __restrict__ dE, int d, int vocab) {
   const int m = blockIdx.x;
   const int id = ids[m];
@@ -1038,6 +1133,34 @@ cudaError_t bias_grad(const bf16* dy, int64_t ld, int M, int n, bf16* db, int ac
       (reinterpret_cast<uintptr_t>(db) & 3))
     return cudaErrorInvalidValue;
   bias_grad_kernel<<<(n + 63) / 64, 256, 0, s>>>(dy, ld, M, n, db, accumulate);
+  return cudaGetLastError();
+}
+namespace {
+bool qk_norm_args_ok(const void* x, int64_t ld, const void* y, int64_t ldy, int M, int q_cols, int n_cols, const bf16* wq, const bf16* wk,
+                     float eps) {
+  return x && y && wq && wk && M > 0 && n_cols > 0 && !(n_cols & 127) && q_cols >= 0 && !(q_cols & 127) && q_cols <= n_cols &&
+         ld >= n_cols && ldy >= n_cols && !(ld & 3) && !(ldy & 3) && !(reinterpret_cast<uintptr_t>(x) & 7) &&
+         !(reinterpret_cast<uintptr_t>(y) & 7) && !(reinterpret_cast<uintptr_t>(wq) & 7) && !(reinterpret_cast<uintptr_t>(wk) & 7) &&
+         eps >= 0.f;
+}
+int qk_norm_grid(int M, int n_cols) {
+  const long long warps = static_cast<long long>(M) * (n_cols >> 7);
+  return static_cast<int>(std::min<long long>((warps + 7) / 8, QKN_MAX_BLOCKS));
+}
+}  // namespace
+cudaError_t qk_norm_fwd(bf16* qkv, int64_t ld, int M, int q_cols, int n_cols, const bf16* wq, const bf16* wk, float eps, bf16* pre,
+                        int64_t ld_pre, cudaStream_t s) {
+  if (!qk_norm_args_ok(qkv, ld, pre, ld_pre, M, q_cols, n_cols, wq, wk, eps)) return cudaErrorInvalidValue;
+  qk_norm_fwd_kernel<<<qk_norm_grid(M, n_cols), 256, 0, s>>>(qkv, ld, M, q_cols, n_cols, wq, wk, eps, pre, ld_pre);
+  return cudaGetLastError();
+}
+cudaError_t qk_norm_bwd(bf16* dy, int64_t ld, const bf16* x, int64_t ldx, int M, int q_cols, int n_cols, const bf16* wq, const bf16* wk,
+                        float eps, bf16* dw, float* scratch, int nblk, int accumulate, cudaStream_t s) {
+  if (!qk_norm_args_ok(dy, ld, x, ldx, M, q_cols, n_cols, wq, wk, eps)) return cudaErrorInvalidValue;
+  if (dw && (!scratch || nblk < 1)) return cudaErrorInvalidValue;
+  const int grid = dw ? nblk : qk_norm_grid(M, n_cols);
+  qk_norm_bwd_kernel<<<grid, 256, 0, s>>>(dy, ld, x, ldx, M, q_cols, n_cols, wq, wk, eps, dw ? scratch : nullptr);
+  if (dw) qk_norm_dw_kernel<<<256 / 32, 256, 0, s>>>(scratch, nblk, dw, accumulate);
   return cudaGetLastError();
 }
 cudaError_t embedding_bwd(const int32_t* ids, const bf16* dx, float* dE32, int M, int d, int vocab, cudaStream_t s) {

@@ -50,6 +50,9 @@ struct GemmKParams {
   const int32_t* m_eff;  // device-side row count; 256-row blocks that start at or beyond it are skipped
   int c_cols, x_cols;    // inner extents of the tmC / tmX tensor maps: output boxes at or beyond them are not issued
   const bf16* bias;      // BIAS kernels: bf16 [N], added to the accumulator before rounding / rotary
+  const bf16 *qk_wq, *qk_wk;  // QKNORM kernels: the [128] q_norm / k_norm weights (columns < qk_q_cols / the rotated ones beyond)
+  int qk_q_cols;
+  float qk_eps;
 };
 
 template <int BN>
@@ -63,7 +66,8 @@ struct GemmCfg {
   static constexpr int STG_BYTES = 2 * 2 * BOX_BYTES;    // two boxes per consumer warpgroup
   // 230 656 of the 232 448 bytes a block may opt into
   static constexpr int SMEM_BYTES = RING_BYTES + STG_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
-  // BIAS kernels: each consumer warpgroup stages the tile's BN bias values behind the barriers (231 680 bytes at BN = 256)
+  // BIAS kernels: each consumer warpgroup stages the tile's BN bias values behind the barriers (231 680 bytes at BN = 256);
+  // QKNORM kernels keep the 2 x 128 norm weights there
   static constexpr int BIAS_BYTES = 2 * BN * 2;
 };
 
@@ -75,7 +79,12 @@ __device__ __forceinline__ float round_bf16(float x) { return __bfloat162float(_
 // consumer warpgroup copies the tile's slice into its own shared-memory row at the start of the tile (one coalesced load per thread,
 // hidden under the main loop); the first pass_begin() barrier of the epilogue orders it before the reads, the last pass_store()
 // barrier of the previous tile orders the previous tile's reads before it.
-template <int BN, bool A_MN, bool B_MN, int EPI, bool BIAS = false>
+// QKNORM (EPI_ROPE only): every rotated 128-column head is RMS-normalised before the rotary (Qwen3 q_norm / k_norm):
+// x = bf16(acc), y = (w * x) * rsqrt(mean(x^2) + eps) in fp32, then the rotary.  A row's 128 values sit in the four lanes of a
+// quad (32 each): 32 products and two shfl.xor give the sum of squares.  The pre-norm x is stored to tmX (aux [M, rope_cols])
+// in an extra pass before the normalised head goes to C.  The two weight vectors sit in the warpgroup's bias row (read with
+// ld.shared: with __ldg the compiler hoists the loads and the epilogue spills).
+template <int BN, bool A_MN, bool B_MN, int EPI, bool BIAS = false, bool QKNORM = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
             const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
@@ -83,6 +92,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   using Cfg = GemmCfg<BN>;
   static_assert(EPI < EPI_ROPE || BN == 256, "the fused epilogues pair columns 64 / 128 apart inside one 256-column tile");
   static_assert(!BIAS || EPI == EPI_BF16 || EPI == EPI_ROPE, "the bias is added by the EPI_BF16 and EPI_ROPE epilogues only");
+  static_assert(!QKNORM || (EPI == EPI_ROPE && !BIAS), "the q/k norm runs in the EPI_ROPE epilogue, without a bias");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::RING_BYTES + Cfg::STG_BYTES);
@@ -186,6 +196,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     int stage = 0;
     uint32_t phase = 0;
     float acc[BN / 2];
+    if (QKNORM) {  // [q_norm | k_norm] weights in this warpgroup's bias row, once for all tiles
+      for (int c = threadIdx.x & 127; c < 256; c += 128) bias_s[c] = c < 128 ? __ldg(p.qk_wq + c) : __ldg(p.qk_wk + c - 128);
+      named_bar_sync(1 + cw, 128);
+    }
 
     // staging address of this thread's element pair in row wq * 16 + rq + 8 * hr of box `box`: 16-byte chunk `ch`, byte `b`
     auto sa = [&](int hr, int box, int ch, int b) -> uint32_t {
@@ -323,6 +337,39 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         }
 #pragma unroll
         for (int hh = 0; hh < 2; ++hh) {
+          float rstd[2] = {1.f, 1.f};
+          if (QKNORM && rot) {
+            // extra pass: the pre-norm bf16 head x to aux, its sum of squares per row, and w * x in place of acc (the rotary
+            // pass below scales by rstd: HF order, q = q_norm(x W^T), then the rotary)
+            const uint32_t w_u = smem_u32(bias_s + (n0 + 128 * hh < p.qk_q_cols ? 0 : 128)) + cq * 2;
+            float ss[2] = {0.f, 0.f};
+            pass_begin();
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+              const int jl = hh * 16 + jj, jh = jl + 8;
+              const float2 wl = unpack_bf16x2(lds32(w_u + jj * 16)), wh = unpack_bf16x2(lds32(w_u + 128 + jj * 16));
+#pragma unroll
+              for (int hr = 0; hr < 2; ++hr) {
+                float* l = acc + 4 * jl + 2 * hr;
+                float* h = acc + 4 * jh + 2 * hr;
+                const float l0 = round_bf16(l[0]), l1 = round_bf16(l[1]), h0 = round_bf16(h[0]), h1 = round_bf16(h[1]);
+                ss[hr] += l0 * l0 + l1 * l1 + h0 * h0 + h1 * h1;
+                sts32(sa(hr, 0, jj, cq * 2), pack_bf16x2(l0, l1));
+                sts32(sa(hr, 1, jj, cq * 2), pack_bf16x2(h0, h1));
+                l[0] = wl.x * l0;
+                l[1] = wl.y * l1;
+                h[0] = wh.x * h0;
+                h[1] = wh.y * h1;
+              }
+            }
+            pass_store(&tmX, p.x_cols, n0 + 128 * hh, 64, 2, y0, 0);
+#pragma unroll
+            for (int hr = 0; hr < 2; ++hr) {
+              ss[hr] += __shfl_xor_sync(0xffffffffu, ss[hr], 1);
+              ss[hr] += __shfl_xor_sync(0xffffffffu, ss[hr], 2);
+              rstd[hr] = rsqrtf(ss[hr] * (1.f / 128.f) + p.qk_eps);
+            }
+          }
           pass_begin();
 #pragma unroll
           for (int jj = 0; jj < 8; ++jj) {
@@ -330,6 +377,12 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 #pragma unroll
             for (int hr = 0; hr < 2; ++hr) {
               float lo[2] = {acc[4 * jl + 2 * hr], acc[4 * jl + 2 * hr + 1]}, hi[2] = {acc[4 * jh + 2 * hr], acc[4 * jh + 2 * hr + 1]};
+              if (QKNORM && rot) {
+                lo[0] *= rstd[hr];
+                lo[1] *= rstd[hr];
+                hi[0] *= rstd[hr];
+                hi[1] *= rstd[hr];
+              }
               if (BIAS) {  // HF order: q = x W^T + b, then the rotary
                 const float2 bl = bias2(jl), bh = bias2(jh);
                 lo[0] += bl.x;
@@ -504,11 +557,11 @@ struct DeviceOnce {
 int g_wide_tiles = 1;
 int g_group_m = GROUP_M;
 
-template <int BN, bool A_MN, bool B_MN, int EPI, bool BIAS = false>
+template <int BN, bool A_MN, bool B_MN, int EPI, bool BIAS = false, bool QKNORM = false>
 cudaError_t launch(const GemmArgs& a, cudaStream_t s) {
   using Cfg = GemmCfg<BN>;
-  constexpr int SMEM = Cfg::SMEM_BYTES + (BIAS ? Cfg::BIAS_BYTES : 0);
-  auto kern = gemm_kernel<BN, A_MN, B_MN, EPI, BIAS>;
+  constexpr int SMEM = Cfg::SMEM_BYTES + (BIAS || QKNORM ? Cfg::BIAS_BYTES : 0);
+  auto kern = gemm_kernel<BN, A_MN, B_MN, EPI, BIAS, QKNORM>;
   static DeviceOnce attr;  // the attribute is per device: a second trainer on another GPU of the same process needs it too
   if (cudaError_t e = attr.run([&] { return cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM); });
       e != cudaSuccess)
@@ -542,6 +595,9 @@ cudaError_t launch(const GemmArgs& a, cudaStream_t s) {
     ok &= make_tmap_2d_bf16(&tX, a.R, x_cols, a.M, a.ldr, 64, 64);
   } else if (EPI == EPI_SWIGLU_FWD || EPI == EPI_SWIGLU_BWD) {
     x_cols = EPI == EPI_SWIGLU_FWD ? a.N / 2 : 2 * a.N;  // act out / gu in
+    ok &= make_tmap_2d_bf16(&tX, a.aux, x_cols, a.M, a.ld_aux, 64, 64);
+  } else if (QKNORM) {  // pre-norm q|k out
+    x_cols = a.rope_cols;
     ok &= make_tmap_2d_bf16(&tX, a.aux, x_cols, a.M, a.ld_aux, 64, 64);
   } else {
     tX = tC;
@@ -578,6 +634,10 @@ cudaError_t launch(const GemmArgs& a, cudaStream_t s) {
   p.c_cols = c_cols;
   p.x_cols = x_cols;
   p.bias = a.bias;
+  p.qk_wq = a.qk_wq;
+  p.qk_wk = a.qk_wk;
+  p.qk_q_cols = a.qk_q_cols;
+  p.qk_eps = a.qk_eps;
   int total = p.m_tiles * p.n_tiles * p.split_k;
   int grid = total < gemm_num_sms() ? total : gemm_num_sms();
   if (grid <= 0) return cudaSuccess;
@@ -598,6 +658,7 @@ cudaError_t launch_epi(const GemmArgs& a, cudaStream_t s) {
 template <bool B_MN>
 cudaError_t launch_fused(const GemmArgs& a, cudaStream_t s) {
   if (a.bias) return a.epilogue == EPI_ROPE ? launch<256, false, B_MN, EPI_ROPE, true>(a, s) : cudaErrorInvalidValue;
+  if (a.qk_wq) return a.epilogue == EPI_ROPE ? launch<256, false, B_MN, EPI_ROPE, false, true>(a, s) : cudaErrorInvalidValue;
   switch (a.epilogue) {
     case EPI_ROPE: return launch<256, false, B_MN, EPI_ROPE>(a, s);
     case EPI_SWIGLU_FWD: return launch<256, false, B_MN, EPI_SWIGLU_FWD>(a, s);
@@ -628,6 +689,12 @@ cudaError_t gemm_bf16(const GemmArgs& a, cudaStream_t s) {
   if (a.epilogue == EPI_BF16_ADD && a.R == nullptr) return cudaErrorInvalidValue;
   // bias variants: the plain bf16 and the RoPE epilogue, K-major A, one split
   if (a.bias && ((a.epilogue != EPI_BF16 && a.epilogue != EPI_ROPE) || a.a_mn_major || a.split_k > 1)) return cudaErrorInvalidValue;
+  // q/k norm: EPI_ROPE only, without a bias; whole heads on both sides of the q / k boundary, a 16-byte aligned pre-norm output
+  if (a.qk_wq && (a.epilogue != EPI_ROPE || a.bias || !a.qk_wk || (a.qk_q_cols & 127) || a.qk_q_cols < 0 ||
+                  a.qk_q_cols > a.rope_cols || !(a.qk_eps >= 0.f) || !a.aux || (a.ld_aux & 7) || a.ld_aux < a.rope_cols ||
+                  (reinterpret_cast<uintptr_t>(a.aux) & 15) || (reinterpret_cast<uintptr_t>(a.qk_wq) & 3) ||
+                  (reinterpret_cast<uintptr_t>(a.qk_wk) & 3)))
+    return cudaErrorInvalidValue;
   // TMA needs 16-byte aligned bases and row strides
   if ((a.lda & 7) || (a.ldb & 7) || (reinterpret_cast<uintptr_t>(a.A) & 15) || (reinterpret_cast<uintptr_t>(a.B) & 15))
     return cudaErrorInvalidValue;

@@ -38,6 +38,11 @@ struct GemmArgs {
   const int32_t* rope_pos = nullptr;  // EPI_ROPE, optional [M]: position of every row inside its sequence (packed ragged batches); null: row % rope_S
   // optional bf16 [N] (EPI_BF16 / EPI_ROPE only, K-major A): added to the fp32 accumulator before rounding / rotary (q|k|v biases)
   const bf16* bias = nullptr;
+  // optional (EPI_ROPE only, no bias): Qwen3 q/k RMSNorm of every rotated 128-column head before the rotary, weight qk_wq [128]
+  // for columns < qk_q_cols and qk_wk [128] beyond; the pre-norm bf16 values of columns < rope_cols go to aux (ld_aux)
+  const bf16 *qk_wq = nullptr, *qk_wk = nullptr;
+  int qk_q_cols = 0;
+  float qk_eps = 0.f;
   int M = 0, N = 0, K = 0;
   // optional device-side row count (<= M): 256-row blocks of tiles that start at or beyond it are skipped (rows up to the
   // end of the last live block are still computed).  Lets the lm_head GEMMs run over the unmasked tokens only without a
@@ -184,6 +189,17 @@ cudaError_t rmsnorm_dw(const bf16* dy, const bf16* x, const float* rstd, int M, 
 cudaError_t embedding_bwd(const int32_t* ids, const bf16* dx, float* dE32, int M, int d, int vocab, cudaStream_t s);
 // bias gradient: db[c] (+)= sum_m dy[m, c] (row stride ld; fp32 per-thread partials summed in a fixed order, no atomics)
 cudaError_t bias_grad(const bf16* dy, int64_t ld, int M, int n, bf16* db, int accumulate, cudaStream_t s);
+// Qwen3 q/k RMSNorm over the 128-value heads of columns [0, n_cols) of packed qkv (row stride ld): weight wq [128] for columns
+// < q_cols, wk [128] beyond.  Forward, in place: pre[m, c] = x, x = w * (x * rsqrt(mean(x^2) + eps)) (fp32).
+cudaError_t qk_norm_fwd(bf16* qkv, int64_t ld, int M, int q_cols, int n_cols, const bf16* wq, const bf16* wk, float eps, bf16* pre,
+                        int64_t ld_pre, cudaStream_t s);
+// Backward, in place on dy: dx = rstd * (w*dy - xh * mean(w*dy*xh)), xh = x * rstd recomputed from the saved pre-norm x.
+// dw (optional, bf16 [256] = [d q_norm | d k_norm]) (+)= sums of dy*xh over rows and heads: nblk blocks write fp32 partials to
+// scratch (>= nblk * 256 floats), a second kernel adds them in a fixed order (no atomics).  Without dw the grid is
+// min(QKN_MAX_BLOCKS, heads / 8) and scratch is unused.
+constexpr int QKN_MAX_BLOCKS = 1024;
+cudaError_t qk_norm_bwd(bf16* dy, int64_t ld, const bf16* x, int64_t ldx, int M, int q_cols, int n_cols, const bf16* wq, const bf16* wk,
+                        float eps, bf16* dw, float* scratch, int nblk, int accumulate, cudaStream_t s);
 // dst[i] = (accumulate ? dst[i] : 0) + src[i]   fp32 -> bf16
 cudaError_t add_f32_into_bf16(const float* src, bf16* dst, int64_t n, int accumulate, cudaStream_t s);
 // *out (+)= sum g[i]^2 over a bf16 buffer (two-stage, fixed order; first = 1 overwrites)

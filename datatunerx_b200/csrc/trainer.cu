@@ -149,6 +149,8 @@ struct Layer {
   // wgu: [2F, d] in the GU-interleaved layout (128 gate rows | 128 up rows per 128 features)
   bf16 *wqkv = nullptr, *wo = nullptr, *wgu = nullptr, *wdown = nullptr, *norm1 = nullptr, *norm2 = nullptr;
   bf16* bias = nullptr;  // dtx_model_ext.qkv_bias: [W] q|k|v biases in the row order of wqkv (bf16 also under NF4), else null
+  bf16* qkn = nullptr;   // dtx_model_ext.qk_norm: [2 * 128] q_norm | k_norm weights (bf16 also under NF4), else null
+  bf16* qk_pre = nullptr;  // qk_norm, saved: [M, dq + dkv] q|k projection output before the norm (bf16)
   bf16 *a_cat = nullptr, *b_ext = nullptr;                                               // shadows
   bf16 *h1 = nullptr, *t = nullptr, *qkv = nullptr, *attn = nullptr, *x_mid = nullptr, *gu = nullptr;  // saved
   bf16* hd = nullptr;  // LoRA dropout only: [M, nt*d] dropped copies of h1, one per target (peft: one nn.Dropout per module)
@@ -201,7 +203,7 @@ struct dtx_trainer {
   int last_groups = 1;          // length groups of the last training micro-batch (diagnostics; 0 = packed)
   bool packed = false;          // the batch in d_ids / d_labels is PACKED: sequence b owns rows d_row_start[b] .. d_row_start[b+1])
   bool use_seq_lens = false;    // d_seq_lens holds this batch's true row lengths
-  int dq = 0, dkv = 0, W = 0;  // q width (= hidden), k/v width (n_kv_heads*128), packed qkv row width
+  int dq = 0, dkv = 0, W = 0;  // q / attention width (n_heads*128), k/v width (n_kv_heads*128), packed qkv row width
   int KA = 0;                  // contraction length of the LoRA down-projection: d, or nt*d with dropout
   bool dropout = false;
   TargetInfo tg[3];
@@ -240,6 +242,8 @@ struct dtx_trainer {
   bool full = false;
   bool qkv_bias = false;        // q|k|v biases (Qwen2): Layer::bias; full-parameter SFT keeps them at off_bias of the layer block
   int64_t off_bias = 0;
+  bool qk_norm = false;         // q/k RMSNorm (Qwen3): Layer::qkn, Layer::qk_pre; full-parameter SFT keeps the weights at off_qkn
+  int64_t off_qkn = 0;
   int64_t layer_elems = 0, glob_elems = 0;
   int64_t off_wo = 0, off_wgu = 0, off_wdown = 0, off_n1 = 0, off_n2 = 0, goff_lm = 0, goff_nf = 0, layer_used = 0, glob_used = 0;
   bf16 *w_flat = nullptr, *g_flat = nullptr;
@@ -267,6 +271,7 @@ struct dtx_trainer {
   // (q, k, v, o, gate, up, down, norm1, norm2); a step with a hole in this map would train on uninitialised memory
   std::vector<uint8_t> loaded;
   std::vector<uint8_t> bias_loaded;  // qkv_bias: q, k, v bias of every layer
+  std::vector<uint8_t> qkn_loaded;   // qk_norm: q_norm, k_norm weight of every layer
   bool all_random = false;
   bool have_lora = false;
   cudaEvent_t ev_fb = nullptr, ev_ar = nullptr;
@@ -336,6 +341,11 @@ struct dtx_trainer {
     for (size_t i = 0; i < bias_loaded.size(); ++i)
       if (!bias_loaded[i]) {
         snprintf(buf, n, "model.layers.%zu.%s.bias", i / 3, per[i % 3]);
+        return buf;
+      }
+    for (size_t i = 0; i < qkn_loaded.size(); ++i)
+      if (!qkn_loaded[i]) {
+        snprintf(buf, n, "model.layers.%zu.self_attn.%s.weight", i / 2, i % 2 ? "k_norm" : "q_norm");
         return buf;
       }
     return nullptr;
@@ -426,6 +436,7 @@ int create_buffers(dtx_trainer* t) {
   const dtx_model_cfg& mc = t->mc;
   const dtx_train_cfg& tc = t->tc;
   const size_t d = mc.hidden, F = mc.ffn, V = mc.vocab, L = mc.n_layers, M = t->M, RP = t->RP, W = t->W, KA = t->KA;
+  const size_t dq = t->dq, QK = t->dq + t->dkv, NQK = 2 * mc.head_dim;  // attention width, q|k width, q_norm | k_norm
   bool ok = true;
   const bool full = t->full;
   if (full) {
@@ -433,7 +444,7 @@ int create_buffers(dtx_trainer* t) {
     const size_t unit = static_cast<size_t>(t->world) * 128;
     auto pad = [&](size_t n) { return (n + unit - 1) / unit * unit; };
     t->off_wo = W * d;
-    t->off_wgu = t->off_wo + d * d;
+    t->off_wgu = t->off_wo + d * dq;
     t->off_wdown = t->off_wgu + 2 * F * d;
     t->off_n1 = t->off_wdown + d * F;
     t->off_n2 = t->off_n1 + d;
@@ -441,6 +452,10 @@ int create_buffers(dtx_trainer* t) {
     if (t->qkv_bias) {  // no weight decay either (HF get_decay_parameter_names excludes "bias"): inside the block's no-decay tail
       t->off_bias = t->layer_used;
       t->layer_used += W;
+    }
+    if (t->qk_norm) {  // the same for the q/k norm weights (HF excludes "_norm." names from weight decay)
+      t->off_qkn = t->layer_used;
+      t->layer_used += NQK;
     }
     t->layer_elems = pad(t->layer_used);
     t->goff_lm = V * d;
@@ -471,6 +486,7 @@ int create_buffers(dtx_trainer* t) {
   t->base_bytes = static_cast<int64_t>((2 * V * d + d) * sizeof(bf16));
   t->loaded.assign(3 + 9 * L, 0);
   t->bias_loaded.assign(t->qkv_bias ? 3 * L : 0, 0);
+  t->qkn_loaded.assign(t->qk_norm ? 2 * L : 0, 0);
   t->layers.resize(L);
   t->xs.resize(L + 1);
   for (size_t l = 0; l <= L; ++l) ok = ok && t->alloc(&t->xs[l], M * d);
@@ -481,23 +497,28 @@ int create_buffers(dtx_trainer* t) {
       y.wqkv = blk; y.wo = blk + t->off_wo; y.wgu = blk + t->off_wgu; y.wdown = blk + t->off_wdown;
       y.norm1 = blk + t->off_n1; y.norm2 = blk + t->off_n2;
       if (t->qkv_bias) y.bias = blk + t->off_bias;
+      if (t->qk_norm) y.qkn = blk + t->off_qkn;
     } else {
-      ok = ok && t->alloc(&y.wqkv, W * d) && t->alloc(&y.wo, d * d) && t->alloc(&y.wgu, 2 * F * d) &&
+      ok = ok && t->alloc(&y.wqkv, W * d) && t->alloc(&y.wo, d * dq) && t->alloc(&y.wgu, 2 * F * d) &&
            t->alloc(&y.wdown, d * F) && t->alloc(&y.norm1, d) && t->alloc(&y.norm2, d);
       if (t->qkv_bias) ok = ok && t->alloc(&y.bias, W);
+      if (t->qk_norm) ok = ok && t->alloc(&y.qkn, NQK);
       y.a_cat = t->a_cat_all + l * RP * KA;
       y.b_ext = t->b_ext_all + l * W * RP;
     }
-    t->base_bytes += static_cast<int64_t>((W * d + d * d + 3 * F * d + 2 * d + (t->qkv_bias ? W : 0)) * sizeof(bf16));
+    t->base_bytes +=
+        static_cast<int64_t>((W * d + d * dq + 3 * F * d + 2 * d + (t->qkv_bias ? W : 0) + (t->qk_norm ? NQK : 0)) * sizeof(bf16));
     if (t->recompute == RECOMPUTE_LAYER && l > 0) {  // one saved set, refilled layer by layer
       const Layer& y0 = t->layers[0];
       y.h1 = y0.h1; y.t = y0.t; y.hd = y0.hd; y.qkv = y0.qkv; y.attn = y0.attn; y.x_mid = y0.x_mid; y.gu = y0.gu;
+      y.qk_pre = y0.qk_pre;
       y.lse = y0.lse; y.rstd1 = y0.rstd1; y.rstd2 = y0.rstd2;
       continue;
     }
     if (!full) ok = ok && t->alloc(&y.t, M * RP);
     ok = ok && t->alloc(&y.h1, M * d) && t->alloc(&y.qkv, M * W) &&
-         t->alloc(&y.attn, M * d) && t->alloc(&y.x_mid, M * d) && t->alloc(&y.gu, M * 2 * F);
+         t->alloc(&y.attn, M * dq) && t->alloc(&y.x_mid, M * d) && t->alloc(&y.gu, M * 2 * F);
+    if (t->qk_norm) ok = ok && t->alloc(&y.qk_pre, M * QK);
     if (t->dropout) ok = ok && t->alloc(&y.hd, M * KA);
     ok = ok && t->alloc(&y.lse, static_cast<size_t>(tc.micro_batch) * mc.n_heads * tc.seq_len) && t->alloc(&y.rstd1, M) &&
          t->alloc(&y.rstd2, M);
@@ -513,7 +534,7 @@ int create_buffers(dtx_trainer* t) {
     CKM(t->zero(t->adam_v, t->n_train));
   }
   ok = ok && t->alloc(&t->h2, M * d) && t->alloc(&t->act, M * F) && t->alloc(&t->dact, M * F) && t->alloc(&t->dgu, M * 2 * F) &&
-       t->alloc(&t->dx_a, M * d) && t->alloc(&t->dx_b, M * d) && t->alloc(&t->dh, M * d) && t->alloc(&t->dattn, M * d) &&
+       t->alloc(&t->dx_a, M * d) && t->alloc(&t->dx_b, M * d) && t->alloc(&t->dh, M * d) && t->alloc(&t->dattn, M * dq) &&
        t->alloc(&t->dqkv, M * W) && (full || t->alloc(&t->dt, M * RP)) && t->alloc(&t->dlogits, M * V) && t->alloc(&t->logits, M * V) &&
        t->alloc(&t->rstdf, M) && t->alloc(&t->row_loss, M) &&
        t->alloc(&t->delta, static_cast<size_t>(tc.micro_batch) * mc.n_heads * tc.seq_len);
@@ -590,7 +611,7 @@ int refresh_shadows(dtx_trainer* t) {
 int nf4_expand(dtx_trainer* t, int l, int which, cudaStream_t s) {
   Layer& y = t->layers[l];
   const int64_t d = t->mc.hidden, F = t->mc.ffn;
-  const int64_t n[4] = {static_cast<int64_t>(t->W) * d, d * d, 2 * F * d, d * F};
+  const int64_t n[4] = {static_cast<int64_t>(t->W) * d, d * t->dq, 2 * F * d, d * F};
   CK(nf4_dequant_bf16(y.q4[which], y.absmax[which], t->scratch_w[which], n[which], s), 1);
   return DTX_OK;
 }
@@ -699,7 +720,7 @@ int layer_fwd(dtx_trainer* t, int l, int phase, bool backward) {
   const dtx_model_cfg& mc = t->mc;
   const dtx_train_cfg& tc = t->tc;
   const int d = mc.hidden, F = mc.ffn, M = t->cur_M, RP = t->RP, H = mc.n_heads, D = mc.head_dim;
-  const int Hkv = mc.n_kv_heads, W = t->W;
+  const int Hkv = mc.n_kv_heads, W = t->W, dq = t->dq, QK = t->dq + t->dkv;
   const int B = t->cur_B, S = t->cur_S;
   const int32_t* seq_lens = t->use_seq_lens ? t->d_seq_lens : nullptr;
   cudaStream_t s = t->stream;
@@ -709,6 +730,8 @@ int layer_fwd(dtx_trainer* t, int l, int phase, bool backward) {
   const bool drop = lora && t->dropout;  // adapters laid out for per-target dropped inputs (KA = nt*d)
   const float p_drop = backward ? tc.lora_dropout : 0.f;  // eval (model.eval()) runs the same path with p = 0
   Layer& y = t->layers[l];
+  const bf16* qk_wq = y.qkn;  // q_norm | k_norm (Qwen3), else null
+  const bf16* qk_wk = y.qkn ? y.qkn + D : nullptr;
   wait_weights(t, l);
   CK(rmsnorm_fwd(t->xs[l], y.norm1, y.h1, y.rstd1, M, d, mc.rms_eps, s), 1);
   const bf16* lora_in = y.h1;
@@ -732,10 +755,14 @@ int layer_fwd(dtx_trainer* t, int l, int phase, bool backward) {
     if (fused) {  // rotary embedding of q and k applied to the fp32 accumulator in the epilogue
       g.epilogue = EPI_ROPE; g.rope_cs = t->rope_cs; g.rope_S = S; g.rope_cols = t->dq + t->dkv;
       g.rope_pos = t->packed ? t->d_pos : nullptr;  // packed batch: a row's position is its offset inside its own sequence
+      if (qk_wq) {  // q/k norm (Qwen3) before the rotary; the pre-norm q|k is saved for the backward pass
+        g.qk_wq = qk_wq; g.qk_wk = qk_wk; g.qk_q_cols = dq; g.qk_eps = mc.rms_eps; g.aux = y.qk_pre; g.ld_aux = QK;
+      }
     }
     CK(gemm_bf16(g, s), 1);
   }
   if (!fused && t->packed) return t->fail(DTX_ERR_STATE, "packed batches need the fused RoPE epilogue");
+  if (!fused && qk_wq) CK(qk_norm_fwd(y.qkv, W, M, dq, QK, qk_wq, qk_wk, mc.rms_eps, y.qk_pre, QK, s), 1);
   if (!fused) CK(rope_qk_inplace_table(y.qkv, t->rope_cs, B, S, H + Hkv, W, D, 0, s), 1);
   {
     AttnArgs a;
@@ -747,8 +774,8 @@ int layer_fwd(dtx_trainer* t, int l, int phase, bool backward) {
   {  // x_mid = x + attn * Wo^T
     BASEW(W_O, wo);
     GemmArgs g;
-    g.A = y.attn; g.lda = d; g.B = wo; g.ldb = d; g.C = y.x_mid; g.ldc = d; g.R = t->xs[l]; g.ldr = d;
-    g.M = M; g.N = d; g.K = d; g.epilogue = EPI_BF16_ADD;
+    g.A = y.attn; g.lda = dq; g.B = wo; g.ldb = dq; g.C = y.x_mid; g.ldc = d; g.R = t->xs[l]; g.ldr = d;
+    g.M = M; g.N = d; g.K = dq; g.epilogue = EPI_BF16_ADD;
     CK(gemm_bf16(g, s), 1);
   }
   CK(rmsnorm_fwd(y.x_mid, y.norm2, t->h2, y.rstd2, M, d, mc.rms_eps, s), 1);
@@ -780,7 +807,7 @@ int fwd_bwd(dtx_trainer* t, bool backward) {
   const dtx_model_cfg& mc = t->mc;
   const dtx_train_cfg& tc = t->tc;
   const int d = mc.hidden, F = mc.ffn, V = mc.vocab, L = mc.n_layers, M = t->cur_M, RP = t->RP, H = mc.n_heads, D = mc.head_dim;
-  const int Hkv = mc.n_kv_heads, W = t->W;
+  const int Hkv = mc.n_kv_heads, W = t->W, dq = t->dq, QK = t->dq + t->dkv;
   const int B = t->cur_B, S = t->cur_S;
   const int32_t* seq_lens = t->use_seq_lens ? t->d_seq_lens : nullptr;
   const int kb_tok = (M + 63) / 64;
@@ -888,11 +915,11 @@ int fwd_bwd(dtx_trainer* t, bool backward) {
     {  // dattn = dx_mid * Wo
       BASEW(W_O, wo);
       GemmArgs g;
-      g.A = other; g.lda = d; g.B = wo; g.ldb = d; g.b_mn_major = 1; g.C = t->dattn; g.ldc = d;
-      g.M = M; g.N = d; g.K = d; g.epilogue = EPI_BF16;
+      g.A = other; g.lda = d; g.B = wo; g.ldb = dq; g.b_mn_major = 1; g.C = t->dattn; g.ldc = dq;
+      g.M = M; g.N = dq; g.K = d; g.epilogue = EPI_BF16;
       CK(gemm_bf16(g, s), 1);
     }
-    if (t->full) CK(dw_gemm(other, d, y.attn, d, gl_w + t->off_wo), 1);  // dWo = d x_mid^T * attn
+    if (t->full) CK(dw_gemm(other, d, y.attn, dq, gl_w + t->off_wo), 1);  // dWo = d x_mid^T * attn
     {
       AttnArgs a;
       a.qkv = y.qkv; a.out = y.attn; a.lse = y.lse; a.B = B; a.S = S; a.H = H; a.Hkv = Hkv; a.scale = att_scale;
@@ -906,6 +933,12 @@ int fwd_bwd(dtx_trainer* t, bool backward) {
       a.rope_cs = rope_in_attn ? t->rope_cs_t : nullptr;
       CK(attn_bwd(a, s), attn_bwd_launches());
       if (!rope_in_attn) CK(rope_qk_inplace_table(t->dqkv, t->rope_cs, B, S, H + Hkv, W, D, 1, s), 1);
+    }
+    if (y.qkn) {  // through the q/k norm (Qwen3), in place on the q|k columns of dqkv; full-parameter SFT: d q_norm | d k_norm
+      // the dw partials: at most as many 256-float blocks as ndw_scratch (64 * d floats) holds
+      const int nblk = std::min(QKN_MAX_BLOCKS, 64 * d / 256);
+      CK(qk_norm_bwd(t->dqkv, W, y.qk_pre, QK, M, dq, QK, y.qkn, y.qkn + D, mc.rms_eps, t->full ? gl_w + t->off_qkn : nullptr,
+                     t->ndw_scratch, nblk, accumulate, s), t->full ? 2 : 1);
     }
     if (lora) {  // dt = dqkv * B_ext   [M, RP]
       GemmArgs g;
@@ -1149,15 +1182,15 @@ bool plan_packed(const dtx_trainer* t, const int32_t* lens, int S_batch, RowStar
   return packed_rows(lens, B, S_batch, rs);
 }
 
-struct PlanDims { int hidden, ffn, W, n_sms, B; };  // what the cost model needs of the model / device / batch
+struct PlanDims { int hidden, ffn, W, dq, n_sms, B; };  // what the cost model needs of the model / device / batch
 
 double group_cost(const PlanDims& t, int rows, int S) {
-  const int d = t.hidden, F = t.ffn, W = t.W;
+  const int d = t.hidden, F = t.ffn, W = t.W, dq = t.dq;
   const long long mt = (static_cast<long long>(rows) * S + 127) / 128;
   const long long slots = std::max(1, t.n_sms);
   auto waves = [&](int n_cols, int k) { return static_cast<double>((mt * ((n_cols + 255) / 256) + slots - 1) / slots) * k; };
   // forward: qkv, o, gate|up, down; backward dX: through down (N = F), gate|up, o, qkv
-  return waves(W, d) + waves(d, d) + waves(2 * F, d) + waves(d, F) + waves(F, d) + waves(d, 2 * F) + waves(d, d) + waves(d, W);
+  return waves(W, d) + waves(d, dq) + waves(2 * F, d) + waves(d, F) + waves(F, d) + waves(d, 2 * F) + waves(dq, d) + waves(d, W);
 }
 
 // labels may be null (planning only: n_div stays 0)
@@ -1336,7 +1369,6 @@ int check_cfg(const dtx_model_cfg* mc, const dtx_train_cfg* tc) {
   };
   if (mc->head_dim != 128) return bad("only head_dim 128 is implemented (Llama-2 / Mistral family)");
   if (mc->n_kv_heads <= 0 || mc->n_heads % mc->n_kv_heads) return bad("n_heads must be a multiple of n_kv_heads");
-  if (mc->n_heads * mc->head_dim != mc->hidden) return bad("hidden != n_heads * head_dim");
   if (mc->hidden % 64 || mc->ffn % 128 || mc->vocab % 8)
     return bad("hidden must be a multiple of 64, ffn a multiple of 128 (GU-interleaved layout), vocab a multiple of 8");
   if (tc->seq_len % 128 || tc->seq_len <= 0 || tc->micro_batch <= 0) return bad("seq_len must be a positive multiple of 128");
@@ -1358,6 +1390,7 @@ int check_ext(const dtx_model_ext* ext) {
     return DTX_ERR_INVALID;
   };
   if (ext->qkv_bias != 0 && ext->qkv_bias != 1) return bad("qkv_bias must be 0 or 1");
+  if (ext->qk_norm != 0 && ext->qk_norm != 1) return bad("qk_norm must be 0 or 1");
   if (ext->rope_type < DTX_ROPE_DEFAULT || ext->rope_type > DTX_ROPE_LLAMA3)
     return bad("rope_type must be DTX_ROPE_DEFAULT, DTX_ROPE_LINEAR or DTX_ROPE_LLAMA3 (yarn, dynamic, longrope are not implemented)");
   if (ext->rope_type != DTX_ROPE_DEFAULT && !(ext->rope_factor > 0.0f)) return bad("rope_factor must be > 0");
@@ -1374,6 +1407,7 @@ void setup_dims(dtx_trainer* t, const dtx_model_cfg* mc, const dtx_model_ext* ex
   t->mc = *mc;
   if (ext) t->ext = *ext;
   t->qkv_bias = t->ext.qkv_bias != 0;
+  t->qk_norm = t->ext.qk_norm != 0;
   t->tc = *tc;
   t->world = world;
   t->M = tc->micro_batch * tc->seq_len;
@@ -1698,6 +1732,15 @@ int32_t dtx_load_tensor(dtx_trainer* t, const char* name, const void* host, int3
       return rc;
     }
   }
+  for (int i = 0; i < 2; ++i) {  // q_norm / k_norm [head_dim]: one [2 * head_dim] vector per layer (bf16 also under NF4)
+    if (!strstr(rest, i ? "self_attn.k_norm.weight" : "self_attn.q_norm.weight")) continue;
+    if (!t->qk_norm) return t->fail(DTX_ERR_INVALID, "%s: this trainer was created without q/k norms (dtx_model_ext.qk_norm)", name);
+    const int64_t D = t->mc.head_dim;
+    if (nd != 1 || rows != D) return t->fail(DTX_ERR_INVALID, "%s: expected [%lld]", name, (long long)D);
+    int rc = upload(y.qkn + i * D, D);
+    if (rc == DTX_OK) t->qkn_loaded[2 * static_cast<size_t>(layer) + i] = 1;
+    return rc;
+  }
   if (t->quant4 && !strstr(rest, "layernorm"))
     return t->fail(DTX_ERR_STATE, "%s: the base weights are already NF4-packed; load tensors before dtx_quantize_base", name);
   // gate/up rows go to the GU-interleaved layout: 128 gate rows, then the 128 up rows of the same features, ...
@@ -1746,17 +1789,19 @@ int32_t dtx_init_random_weights(dtx_trainer* t, uint64_t seed) {
   CK(fill_const_bf16(t->normf, d, 1.0f, s), 1);
   for (Layer& y : t->layers) {
     CK(fill_normal_bf16(y.wqkv, static_cast<int64_t>(t->W) * d, 0.02f, ++k, s), 1);
-    CK(fill_normal_bf16(y.wo, d * d, 0.02f, ++k, s), 1);
+    CK(fill_normal_bf16(y.wo, d * t->dq, 0.02f, ++k, s), 1);
     CK(fill_normal_bf16(y.wgu, 2 * F * d, 0.02f, ++k, s), 1);
     CK(fill_normal_bf16(y.wdown, d * F, 0.02f, ++k, s), 1);
     CK(fill_const_bf16(y.norm1, d, 1.0f, s), 1);
     CK(fill_const_bf16(y.norm2, d, 1.0f, s), 1);
     if (y.bias) CK(fill_const_bf16(y.bias, t->W, 0.0f, s), 1);  // HF _init_weights zeroes Linear biases
+    if (y.qkn) CK(fill_const_bf16(y.qkn, 2 * t->mc.head_dim, 1.0f, s), 1);  // ... and sets RMSNorm weights to 1
   }
   cudaError_t e = cudaStreamSynchronize(s);
   if (e != cudaSuccess) return t->fail(DTX_ERR_CUDA, "init_random_weights: %s", cudaGetErrorString(e));
   std::fill(t->loaded.begin(), t->loaded.end(), 1);
   std::fill(t->bias_loaded.begin(), t->bias_loaded.end(), 1);
+  std::fill(t->qkn_loaded.begin(), t->qkn_loaded.end(), 1);
   return DTX_OK;
 }
 
@@ -1777,7 +1822,7 @@ int32_t dtx_quantize_base(dtx_trainer* t, int32_t mode) {
   }
   cudaSetDevice(t->device);
   const int64_t d = t->mc.hidden, F = t->mc.ffn, W = t->W;
-  const int64_t n[4] = {W * d, d * d, 2 * F * d, d * F};
+  const int64_t n[4] = {W * d, d * t->dq, 2 * F * d, d * F};
   for (int i = 0; i < 4; ++i)
     if (n[i] % 64) return t->fail(DTX_ERR_INVALID, "quantize_base: matrix sizes must be multiples of the 64-element NF4 block");
   cudaStream_t s = t->stream;
@@ -1863,7 +1908,7 @@ int32_t dtx_step(dtx_trainer* t, const int32_t* ids, const int32_t* labels, cons
     return rc;
   }
   SubPlan plan;
-  if (!t->full) plan_groups(PlanDims{t->mc.hidden, t->mc.ffn, t->W, t->n_sms, t->tc.micro_batch}, seq_lens, labels, t->cur_S, &plan);
+  if (!t->full) plan_groups(PlanDims{t->mc.hidden, t->mc.ffn, t->W, t->dq, t->n_sms, t->tc.micro_batch}, seq_lens, labels, t->cur_S, &plan);
   if (plan.n > 1) {  // ragged batch: the whole batch goes to the staging buffers, the length groups gather from there
     const int S_src = t->cur_S;
     CKM(cudaMemcpyAsync(t->d_ids_full, ids, static_cast<size_t>(t->cur_M) * 4, cudaMemcpyHostToDevice, t->stream));
@@ -1909,7 +1954,7 @@ int32_t dtx_step_device(dtx_trainer* t, const void* d_ids, const void* d_labels,
     CKM(cudaMemcpyAsync(t->h_labels.data(), d_labels, t->h_labels.size() * 4, cudaMemcpyDeviceToHost, t->stream));
     CKM(cudaStreamSynchronize(t->stream));
     SubPlan plan;
-    plan_groups(PlanDims{t->mc.hidden, t->mc.ffn, t->W, t->n_sms, t->tc.micro_batch}, t->h_lens.data(), t->h_labels.data(), t->cur_S, &plan);
+    plan_groups(PlanDims{t->mc.hidden, t->mc.ffn, t->W, t->dq, t->n_sms, t->tc.micro_batch}, t->h_lens.data(), t->h_labels.data(), t->cur_S, &plan);
     if (plan.n > 1)
       return do_step(t, flags, loss, gnorm, lr, stepped, &plan, static_cast<const int32_t*>(d_ids), static_cast<const int32_t*>(d_labels),
                      static_cast<const int32_t*>(d_seq_lens), t->cur_S);
@@ -1952,7 +1997,7 @@ int32_t dtx_eval_loss(dtx_trainer* t, const int32_t* ids, const int32_t* labels,
     return DTX_OK;
   }
   SubPlan plan;
-  if (!t->full) plan_groups(PlanDims{t->mc.hidden, t->mc.ffn, t->W, t->n_sms, B}, seq_lens, labels, t->cur_S, &plan);
+  if (!t->full) plan_groups(PlanDims{t->mc.hidden, t->mc.ffn, t->W, t->dq, t->n_sms, B}, seq_lens, labels, t->cur_S, &plan);
   if (plan.n > 1) {
     // ragged batch as length groups (forward only): the per-row statistics come back in group order and are put back in
     // the caller's row order; the batch loss accumulates over the groups with the whole batch's labelled-token count
@@ -2113,7 +2158,7 @@ int32_t dtx_export_weight(dtx_trainer* t, const char* name, void* host_out, int6
   struct Slot { const char* key; int64_t off, n; };
   const Slot slots[] = {
       {"self_attn.q_proj.weight", 0, dq * d}, {"self_attn.k_proj.weight", dq * d, dkv * d},
-      {"self_attn.v_proj.weight", (dq + dkv) * d, dkv * d}, {"self_attn.o_proj.weight", t->off_wo, d * d},
+      {"self_attn.v_proj.weight", (dq + dkv) * d, dkv * d}, {"self_attn.o_proj.weight", t->off_wo, d * dq},
       {"mlp.down_proj.weight", t->off_wdown, d * F}, {"input_layernorm.weight", t->off_n1, d},
       {"post_attention_layernorm.weight", t->off_n2, d},
   };
@@ -2126,6 +2171,11 @@ int32_t dtx_export_weight(dtx_trainer* t, const char* name, void* host_out, int6
     };
     for (const Slot& sl : bias_slots)
       if (strstr(rest, sl.key)) return copy(blk + sl.off, sl.n);
+  }
+  if (t->qk_norm) {
+    const int64_t D = t->mc.head_dim;
+    if (strstr(rest, "self_attn.q_norm.weight")) return copy(blk + t->off_qkn, D);
+    if (strstr(rest, "self_attn.k_norm.weight")) return copy(blk + t->off_qkn + D, D);
   }
   return t->fail(DTX_ERR_INVALID, "unknown tensor name %s", name);
 }
@@ -2171,7 +2221,8 @@ int32_t dtx_plan_length_groups(const dtx_model_cfg* mc, int32_t micro_batch, int
     return DTX_ERR_INVALID;
   const int hkv = mc->n_kv_heads > 0 ? mc->n_kv_heads : mc->n_heads;
   SubPlan plan;
-  plan_groups(PlanDims{mc->hidden, mc->ffn, (mc->n_heads + 2 * hkv) * mc->head_dim, n_sms > 0 ? n_sms : 132, micro_batch}, seq_lens, nullptr,
+  plan_groups(PlanDims{mc->hidden, mc->ffn, (mc->n_heads + 2 * hkv) * mc->head_dim, mc->n_heads * mc->head_dim, n_sms > 0 ? n_sms : 132,
+                       micro_batch}, seq_lens, nullptr,
               seq_len_batch, &plan);
   if (plan.n <= 1) {  // one pass at the batch's padded length, rows in their own order
     for (int i = 0; i < micro_batch; ++i) order_out[i] = i;

@@ -42,7 +42,8 @@ class ModelCfg(C.Structure):
 
 class ModelExt(C.Structure):
     _fields_ = [("qkv_bias", C.c_int32), ("rope_type", C.c_int32), ("rope_factor", C.c_float),
-                ("rope_low_freq_factor", C.c_float), ("rope_high_freq_factor", C.c_float), ("rope_original_max_pos", C.c_int32)]
+                ("rope_low_freq_factor", C.c_float), ("rope_high_freq_factor", C.c_float), ("rope_original_max_pos", C.c_int32),
+                ("qk_norm", C.c_int32)]
 
 
 class TrainCfg(C.Structure):
@@ -57,7 +58,8 @@ class TrainCfg(C.Structure):
 # every symbol include/dtxtune.h declares (tests/test_abi.py checks the .so exports all of them)
 ABI_SYMBOLS = [
     "dtx_abi_version", "dtx_last_global_error", "dtx_last_error", "dtx_trainer_create", "dtx_trainer_create_ext",
-    "dtx_rope_inv_freq", "dtx_plan_device_bytes_ext", "dtx_gemm_bias", "dtx_bias_grad", "dtx_trainer_destroy",
+    "dtx_rope_inv_freq", "dtx_plan_device_bytes_ext", "dtx_gemm_bias", "dtx_bias_grad", "dtx_gemm_qk_norm", "dtx_qk_norm_fwd",
+    "dtx_qk_norm_bwd", "dtx_trainer_destroy",
     "dtx_get_nccl_unique_id", "dtx_load_tensor", "dtx_init_random_weights", "dtx_init_lora", "dtx_quantize_base", "dtx_step",
     "dtx_step_device", "dtx_eval_loss", "dtx_allreduce_host", "dtx_export_adapter", "dtx_export_adapter_grad", "dtx_export_weight", "dtx_num_trainable", "dtx_launch_count",
     "dtx_recompute", "dtx_device_bytes", "dtx_plan_device_bytes",
@@ -93,6 +95,10 @@ def load() -> C.CDLL:
     lib.dtx_gemm_bias.argtypes = [vp, i64, vp, i64, i32, vp, i64, vp, i64, i32, vp, i64, vp, i64, vp, i32, i32, vp, i32, i32, i32,
                                   i32, vp, vp]
     lib.dtx_bias_grad.argtypes = [vp, i64, i32, i32, vp, i32, vp]
+    lib.dtx_gemm_qk_norm.argtypes = [vp, i64, vp, i64, i32, vp, i64, vp, i64, i32, vp, i64, vp, i64, vp, i32, i32, vp, i32, i32, i32,
+                                     i32, vp, vp, C.c_float, vp]
+    lib.dtx_qk_norm_fwd.argtypes = [vp, i64, i32, i32, i32, vp, vp, C.c_float, vp, i64, vp]
+    lib.dtx_qk_norm_bwd.argtypes = [vp, i64, vp, i64, i32, i32, i32, vp, vp, C.c_float, vp, vp, i32, i32, vp]
     lib.dtx_trainer_destroy.argtypes = [vp]
     lib.dtx_trainer_destroy.restype = None
     lib.dtx_get_nccl_unique_id.argtypes = [vp]
@@ -228,6 +234,7 @@ class ModelConfig:
     max_seq: int = 4096
     sliding_window: int = 0            # Mistral config.json `sliding_window`; 0 = none
     qkv_bias: bool = False             # q_proj / k_proj / v_proj carry a bias (Qwen2)
+    qk_norm: bool = False              # RMSNorm over every q / k head before the rotary (Qwen3 q_norm / k_norm)
     # HF config.json `rope_scaling` / `rope_parameters`: {"rope_type" (or the older "type"): "linear" | "llama3", "factor", ...};
     # None = the plain theta table
     rope_scaling: Optional[dict] = None
@@ -245,10 +252,11 @@ class ModelConfig:
         kind = rs.get("rope_type", rs.get("type", "default"))
         if kind not in ROPE_TYPES:
             raise DtxError(-1, f"rope_type {kind!r}: only {', '.join(ROPE_TYPES)} are implemented natively")
+        qkn = int(bool(self.qk_norm))
         if kind == "default":
-            return ModelExt(int(bool(self.qkv_bias)), 0, 0.0, 0.0, 0.0, 0)
+            return ModelExt(int(bool(self.qkv_bias)), 0, 0.0, 0.0, 0.0, 0, qkn)
         return ModelExt(int(bool(self.qkv_bias)), ROPE_TYPES[kind], float(rs["factor"]), float(rs.get("low_freq_factor", 0.0)),
-                        float(rs.get("high_freq_factor", 0.0)), int(rs.get("original_max_position_embeddings", 0)))
+                        float(rs.get("high_freq_factor", 0.0)), int(rs.get("original_max_position_embeddings", 0)), qkn)
 
 
 @dataclass
@@ -408,9 +416,9 @@ class Trainer:
         out = {}
         fn = self.lib.dtx_export_adapter_grad if grads else self.lib.dtx_export_adapter
         d, r = self.model.hidden, self.train.lora_r
-        dkv = (self.model.n_kv_heads or self.model.n_heads) * self.model.head_dim
+        dq, dkv = self.model.n_heads * self.model.head_dim, (self.model.n_kv_heads or self.model.n_heads) * self.model.head_dim
         for name in self.adapter_names():
-            d_out = d if ".q_proj." in name else dkv
+            d_out = dq if ".q_proj." in name else dkv
             shape = (r, d) if "lora_A" in name else (d_out, r)
             buf = np.empty(shape, dtype=np.float32)
             check(fn(self._h, name.encode(), buf.ctypes.data_as(C.c_void_p), buf.nbytes), self._h)
@@ -421,17 +429,21 @@ class Trainer:
         """(HF name, shape) of every tensor of the model, in checkpoint order."""
         m = self.model
         d, F, V, dkv = m.hidden, m.ffn, m.vocab, (m.n_kv_heads or m.n_heads) * m.head_dim
+        dq = m.n_heads * m.head_dim
         yield "model.embed_tokens.weight", (V, d)
         for l in range(m.n_layers):
             p = f"model.layers.{l}."
-            yield p + "self_attn.q_proj.weight", (d, d)
+            yield p + "self_attn.q_proj.weight", (dq, d)
             yield p + "self_attn.k_proj.weight", (dkv, d)
             yield p + "self_attn.v_proj.weight", (dkv, d)
             if m.qkv_bias:
                 yield p + "self_attn.q_proj.bias", (d,)
                 yield p + "self_attn.k_proj.bias", (dkv,)
                 yield p + "self_attn.v_proj.bias", (dkv,)
-            yield p + "self_attn.o_proj.weight", (d, d)
+            if m.qk_norm:
+                yield p + "self_attn.q_norm.weight", (m.head_dim,)
+                yield p + "self_attn.k_norm.weight", (m.head_dim,)
+            yield p + "self_attn.o_proj.weight", (d, dq)
             yield p + "mlp.gate_proj.weight", (F, d)
             yield p + "mlp.up_proj.weight", (F, d)
             yield p + "mlp.down_proj.weight", (d, F)

@@ -1,7 +1,7 @@
 """Model / adapter file IO of the worker, numpy only (no torch, no safetensors package needed at run time).
 
   * load_model_config  : HF config.json -> ModelConfig  (AutoConfig.from_pretrained, cmd/tuning/train.py:221): Llama-2,
-                         Llama-3.x (linear / llama3 rope scaling), Mistral, Qwen2 / Qwen2.5 (q/k/v biases)
+                         Llama-3.x (linear / llama3 rope scaling), Mistral, Qwen2 / Qwen2.5 (q/k/v biases), Qwen3 (q/k norm)
   * iter_safetensors   : stream tensors of *.safetensors shards (AutoModelForCausalLM.from_pretrained, train.py:236-242);
                          iter_torch_bin does the same for pytorch_model*.bin shards
   * save_peft_adapter  : adapter_config.json + adapter_model.safetensors (+ adapter_model.bin when torch is importable)
@@ -29,12 +29,13 @@ _ROPE_TYPES = ("default", "linear", "llama3")
 
 def load_model_config(model_dir: str, full_finetune: bool = False) -> ModelConfig:
     """HF config.json -> ModelConfig for the decoders the library trains: Llama-2 / Llama-3.x (`rope_scaling` of type linear or
-    llama3), Mistral and Qwen2 / Qwen2.5 (q/k/v biases).  Anything that would train a different model than HF's raises ValueError."""
+    llama3), Mistral, Qwen2 / Qwen2.5 (q/k/v biases) and Qwen3 (q/k RMSNorm, attention width n_heads * head_dim != hidden).
+    Anything that would train a different model than HF's raises ValueError."""
     cfg = json.load(open(os.path.join(model_dir, "config.json")))
     arch = (cfg.get("architectures") or ["LlamaForCausalLM"])[0]
-    qwen2 = arch == "Qwen2ForCausalLM"
-    if "Llama" not in arch and "Mistral" not in arch and not qwen2:
-        raise ValueError(f"{arch}: only Llama-family and Qwen2 decoders are implemented natively")
+    qwen2, qwen3 = arch == "Qwen2ForCausalLM", arch == "Qwen3ForCausalLM"
+    if "Llama" not in arch and "Mistral" not in arch and not qwen2 and not qwen3:
+        raise ValueError(f"{arch}: only Llama-family, Qwen2 and Qwen3 decoders are implemented natively")
     if cfg.get("attention_bias") or cfg.get("mlp_bias"):
         raise ValueError(f"{arch}: attention_bias / mlp_bias are not implemented natively")
     # transformers 5 names the dict `rope_parameters` (it then also carries rope_theta); older configs `rope_scaling`
@@ -46,19 +47,21 @@ def load_model_config(model_dir: str, full_finetune: bool = False) -> ModelConfi
             raise ValueError(f"rope_scaling type {kind!r} is not implemented natively (supported: {', '.join(_ROPE_TYPES)})")
         rs = None if kind == "default" else dict(rs)
     window = int(cfg.get("sliding_window") or 0)
-    if qwen2:
-        # Qwen2.5 ships sliding_window = 131072 with use_sliding_window = false: HF then attends over the whole causal window
+    if qwen2 or qwen3:
+        # Qwen2.5 / Qwen3 ship sliding_window with use_sliding_window = false: HF then attends over the whole causal window
+        name = "Qwen2" if qwen2 else "Qwen3"
         if cfg.get("use_sliding_window"):
-            raise ValueError("Qwen2 use_sliding_window (per-layer sliding windows) is not implemented natively")
+            raise ValueError(f"{name} use_sliding_window (per-layer sliding windows) is not implemented natively")
         window = 0
         if full_finetune and cfg.get("tie_word_embeddings"):
-            raise ValueError("full-parameter SFT of a Qwen2 checkpoint with tie_word_embeddings would train the embedding and "
+            raise ValueError(f"full-parameter SFT of a {name} checkpoint with tie_word_embeddings would train the embedding and "
                              "lm_head as two tensors, unlike HF; use LoRA")
     heads = cfg["num_attention_heads"]
     return ModelConfig(vocab=cfg["vocab_size"], hidden=cfg["hidden_size"], n_layers=cfg["num_hidden_layers"], n_heads=heads,
                        n_kv_heads=cfg.get("num_key_value_heads", heads), head_dim=cfg.get("head_dim") or cfg["hidden_size"] // heads,
                        ffn=cfg["intermediate_size"], rms_eps=cfg.get("rms_norm_eps", 1e-5), rope_theta=rope_theta,
-                       max_seq=cfg.get("max_position_embeddings", 4096), sliding_window=window, qkv_bias=qwen2, rope_scaling=rs)
+                       max_seq=cfg.get("max_position_embeddings", 4096), sliding_window=window, qkv_bias=qwen2, qk_norm=qwen3,
+                       rope_scaling=rs)
 
 
 def check_attention_window(model_dir: str, seq_len: int) -> None:

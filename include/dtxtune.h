@@ -87,8 +87,10 @@ typedef struct {
   int32_t recompute;
 } dtx_train_cfg;
 
-/* Model-family extensions of dtx_model_cfg (Llama-3.1 / 3.2 scaled rotary tables, Qwen2 q/k/v projection biases).  A NULL
- * or all-zero dtx_model_ext is the plain Llama-2 / Mistral model: no bias, rotary inverse frequencies theta^(-2i/D). */
+/* Model-family extensions of dtx_model_cfg (Llama-3.1 / 3.2 scaled rotary tables, Qwen2 q/k/v projection biases, Qwen3 q/k
+ * RMSNorm).  A NULL or all-zero dtx_model_ext is the plain Llama-2 / Mistral model: no bias, no q/k norm, rotary inverse
+ * frequencies theta^(-2i/D).  qk_norm was appended after the struct's first release: C callers must be rebuilt against this
+ * header (a caller compiled against the shorter struct passes a struct the library reads one field past). */
 #define DTX_ROPE_DEFAULT 0   /* inv_freq = theta^(-2i/D) */
 #define DTX_ROPE_LINEAR  1   /* inv_freq / factor (HF rope_type "linear") */
 #define DTX_ROPE_LLAMA3  2   /* HF _compute_llama3_parameters (Llama-3.1 / 3.2): high frequencies kept, low ones / factor,
@@ -98,6 +100,7 @@ typedef struct {
   int32_t rope_type;                /* DTX_ROPE_* */
   float rope_factor, rope_low_freq_factor, rope_high_freq_factor;  /* factor: linear and llama3; the two others: llama3 */
   int32_t rope_original_max_pos;    /* llama3: original_max_position_embeddings */
+  int32_t qk_norm;                  /* 1: RMSNorm over every q and k head before the rotary (Qwen3 q_norm / k_norm, eps = rms_eps) */
 } dtx_model_ext;
 
 typedef struct dtx_trainer dtx_trainer;
@@ -113,9 +116,13 @@ DTX_API const char* dtx_last_error(const dtx_trainer* t);
 DTX_API int32_t dtx_trainer_create(const dtx_model_cfg* model, const dtx_train_cfg* train, int32_t device, int32_t rank,
                            int32_t world, const void* nccl_unique_id, dtx_trainer** out);
 /* The same for a model with family extensions (ext may be NULL: dtx_trainer_create).  An unknown rope_type, a factor <= 0, or
- * for llama3 low_freq_factor >= high_freq_factor or original_max_pos <= 0 return DTX_ERR_INVALID before any device work.
+ * for llama3 low_freq_factor >= high_freq_factor or original_max_pos <= 0, or qkv_bias / qk_norm other than 0 / 1 return
+ * DTX_ERR_INVALID before any device work.
  * With qkv_bias, "model.layers.N.self_attn.{q,k,v}_proj.bias" must be loaded before a step; full-parameter SFT trains them
- * without weight decay (HF get_decay_parameter_names), LoRA keeps them frozen (peft bias="none"). */
+ * without weight decay (HF get_decay_parameter_names), LoRA keeps them frozen (peft bias="none").  With qk_norm, the same holds
+ * for "model.layers.N.self_attn.{q,k}_norm.weight" [head_dim].
+ * The attention width n_heads * head_dim need not equal hidden (Qwen3, Mistral-Nemo): q_proj is [n_heads * head_dim, hidden],
+ * o_proj [hidden, n_heads * head_dim]. */
 DTX_API int32_t dtx_trainer_create_ext(const dtx_model_cfg* model, const dtx_model_ext* ext, const dtx_train_cfg* train,
                                        int32_t device, int32_t rank, int32_t world, const void* nccl_unique_id, dtx_trainer** out);
 /* host arithmetic, no device: the fp32 inverse frequencies the rotary table is built from (head_dim / 2 values) */
@@ -260,6 +267,25 @@ DTX_API int32_t dtx_gemm_bias(const void* A, int64_t lda, const void* B, int64_t
 /* bias gradient: db[n] (+)= sum_m dy[m, n] over a bf16 [M, n] matrix with row stride ld (fp32, fixed summation order);
  * accumulate = 0 overwrites db (bf16 [n]) */
 DTX_API int32_t dtx_bias_grad(const void* dy, int64_t ld, int32_t M, int32_t n, void* db, int32_t accumulate, void* stream);
+/* dtx_gemm_bias's arguments for epilogue 3 (EPI_ROPE) without the bias, plus Qwen3's q/k RMSNorm before the rotary: every
+ * rotated 128-column head (columns < rope_cols) becomes (w * x) * rsqrt(mean(x^2) + eps) in fp32, x = the bf16-rounded
+ * projection, w = wq [128] for columns < q_cols, wk [128] beyond.  The pre-norm x of columns < rope_cols goes to aux (row
+ * stride ld_aux).  q_cols and rope_cols: multiples of 128 and 256, N a multiple of 256. */
+DTX_API int32_t dtx_gemm_qk_norm(const void* A, int64_t lda, const void* B, int64_t ldb, int32_t b_mn_major, const void* A2,
+                                 int64_t lda2, const void* B2, int64_t ldb2, int32_t K2, void* C, int64_t ldc, void* aux, int64_t ld_aux,
+                                 const void* rope_cs, int32_t rope_S, int32_t rope_cols, const void* rope_pos, int32_t M, int32_t N,
+                                 int32_t K, int32_t q_cols, const void* wq, const void* wk, float eps, void* stream);
+/* The same norm on its own, in place on columns [0, n_cols) of a bf16 [M, ld] matrix (the unfused path: before the RoPE
+ * kernel); pre (row stride ld_pre) receives the values before the norm. */
+DTX_API int32_t dtx_qk_norm_fwd(void* qkv, int64_t ld, int32_t M, int32_t q_cols, int32_t n_cols, const void* wq, const void* wk,
+                                float eps, void* pre, int64_t ld_pre, void* stream);
+/* Its backward, in place on dy (after the inverse rotary): dx = rstd * (w*dy - xh * mean(w*dy*xh)), xh = x * rstd recomputed
+ * from the saved pre-norm x.  dw (optional, bf16 [256]: d q_norm | d k_norm) (+)= the sums of dy*xh over rows and heads in a
+ * fixed order: nblk (1 .. 1024) blocks of fp32 partials in scratch (>= nblk * 256 floats), then one more kernel adds them.
+ * accumulate = 0 overwrites dw.  With dw NULL, scratch and nblk are ignored. */
+DTX_API int32_t dtx_qk_norm_bwd(void* dy, int64_t ld, const void* x, int64_t ldx, int32_t M, int32_t q_cols, int32_t n_cols,
+                                const void* wq, const void* wk, float eps, void* dw, void* scratch, int32_t nblk, int32_t accumulate,
+                                void* stream);
 DTX_API int32_t dtx_embedding_fwd(const void* ids, const void* table, void* out, int32_t M, int32_t d, int32_t vocab, void* stream);
 DTX_API int32_t dtx_rmsnorm_fwd(const void* x, const void* w, void* y, void* rstd, int32_t M, int32_t d, float eps, void* stream);
 DTX_API int32_t dtx_rmsnorm_bwd(const void* dy, const void* x, const void* w, const void* rstd, const void* dres, void* dx,

@@ -4,8 +4,11 @@
     FFN 18 944, vocab 152 064), random-init weights, LoRA r=16 on q_proj,v_proj, micro-batch 4 x 2048 - the headline bench.py
     workload on the checkpoints people fine-tune today.  Per config: tokens/s of `--runs` timed windows of `--steps` optimizer
     steps (median and range), the activation layout automatic mode chose, the planned and the held device bytes.
-  * The Qwen2.5-7B q|k|v GEMM (M 8192 x N 4608 x K 3584, fused RoPE epilogue) with and without the bias, alternated in one
-    process, timed with CUDA events.
+  * Qwen3-8B shape (q/k RMSNorm, GQA 32 / 8, FFN 12 288, vocab 151 936) and Qwen3-4B shape (hidden 2560 with 32 x 128-wide
+    heads: the attention is wider than the residual stream), the same workload.
+  * The Qwen2.5-7B q|k|v GEMM (M 8192 x N 4608 x K 3584, fused RoPE epilogue) with and without the bias, and the Qwen3-8B one
+    (M 8192 x N 6144 x K 4096) with and without the QK-norm epilogue, each pair alternated in one process, timed with CUDA
+    events; qk_norm_bwd at the Qwen3-8B shape (time and GB/s of the bytes it must move).
 
 The card's name and power limit are read in the same run and printed with the numbers.  Prints one JSON document; --out also
 writes it to a file.
@@ -35,6 +38,10 @@ CONFIGS = {
                                                "original_max_position_embeddings": 8192}),
     "qwen2.5-7b": L.ModelConfig(vocab=152064, hidden=3584, n_layers=28, n_heads=28, n_kv_heads=4, ffn=18944, rope_theta=1000000.0,
                                 rms_eps=1e-6, max_seq=32768, qkv_bias=True),
+    "qwen3-8b": L.ModelConfig(vocab=151936, hidden=4096, n_layers=36, n_heads=32, n_kv_heads=8, ffn=12288, rope_theta=1000000.0,
+                              rms_eps=1e-6, max_seq=40960, qk_norm=True),
+    "qwen3-4b": L.ModelConfig(vocab=151936, hidden=2560, n_layers=36, n_heads=32, n_kv_heads=8, ffn=9728, rope_theta=1000000.0,
+                              rms_eps=1e-6, max_seq=40960, qk_norm=True),
 }
 
 
@@ -108,6 +115,66 @@ def bias_gemm_cost(iters: int, rounds: int) -> dict:
     return res
 
 
+def _alternate(launch, variants, iters: int, rounds: int) -> dict:
+    """ms per launch of every variant (CUDA events over `iters` launches), variants alternated `rounds` times"""
+    import torch
+    for v in variants:
+        for _ in range(10):
+            launch(v)
+    times = {v: [] for v in variants}
+    for _ in range(rounds):
+        for v in variants:
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            for _ in range(iters):
+                launch(v)
+            e1.record()
+            torch.cuda.synchronize()
+            times[v].append(e0.elapsed_time(e1) / iters)
+    return times
+
+
+def qk_norm_cost(iters: int, rounds: int) -> dict:
+    """Qwen3-8B: the q|k|v GEMM with the fused RoPE epilogue with and without QKNORM, and qk_norm_bwd on its dqkv"""
+    import torch
+    M, N, K, H, Hkv, D = 8192, 6144, 4096, 32, 8, 128
+    dq, QK = H * D, (H + Hkv) * D
+    lib = L.load()
+    g = torch.Generator().manual_seed(0)
+    A = (torch.randn(M, K, generator=g) * 0.5).to(torch.bfloat16).cuda()
+    Bw = (torch.randn(N, K, generator=g) * 0.02).to(torch.bfloat16).cuda()
+    wq = (1 + torch.randn(D, generator=g) * 0.1).to(torch.bfloat16).cuda()
+    wk = (1 + torch.randn(D, generator=g) * 0.1).to(torch.bfloat16).cuda()
+    Cm = torch.empty(M, N, dtype=torch.bfloat16, device="cuda")
+    pre = torch.empty(M, QK, dtype=torch.bfloat16, device="cuda")
+    dy = (torch.randn(M, N, generator=g) * 0.1).to(torch.bfloat16).cuda()
+    cs = torch.empty(S_ROPE, D // 2, 2, dtype=torch.float32, device="cuda")
+    stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+    L.check(lib.dtx_rope_table(C.c_void_p(cs.data_ptr()), S_ROPE, D, 1000000.0, stream))
+    P = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None  # noqa: E731
+
+    def gemm(with_norm: bool):
+        L.check(lib.dtx_gemm_qk_norm(P(A), K, P(Bw), K, 0, None, 0, None, 0, 0, P(Cm), N, P(pre), QK, P(cs), S_ROPE, QK, None,
+                                     M, N, K, dq, P(wq), P(wk), 1e-6, stream) if with_norm else
+                lib.dtx_gemm_fused(P(A), K, P(Bw), K, 0, None, 0, None, 0, 0, P(Cm), N, None, 0, P(cs), S_ROPE, QK,
+                                   M, N, K, L.EPI_ROPE, stream))
+
+    times = _alternate(gemm, (False, True), iters, rounds)
+    flop = 2.0 * M * N * K
+    res = {}
+    for wn, key in ((False, "rope"), (True, "rope_qknorm")):
+        ms = statistics.median(times[wn])
+        res[key] = {"ms_median": ms, "ms_range": [min(times[wn]), max(times[wn])], "tflops": flop / ms / 1e9}
+    res["gemm_shape"] = [M, N, K]
+    # backward (LoRA: no dw): reads dy and the pre-norm x of the q|k columns, writes dx
+    bwd = _alternate(lambda _: L.check(lib.dtx_qk_norm_bwd(P(dy), N, P(pre), QK, M, dq, QK, P(wq), P(wk), 1e-6, None, None, 0, 0,
+                                                           stream)), (0,), iters, rounds)[0]
+    ms = statistics.median(bwd)
+    nbytes = 3 * M * QK * 2
+    res["qk_norm_bwd"] = {"ms_median": ms, "ms_range": [min(bwd), max(bwd)], "bytes": nbytes, "gb_per_s": nbytes / ms / 1e6}
+    return res
+
+
 S_ROPE = 2048
 
 
@@ -126,6 +193,7 @@ def main() -> None:
         res["runs"].append(train_throughput(name, CONFIGS[name], a.batch, a.seq, a.steps, a.warmup, a.runs))
         print(json.dumps(res["runs"][-1]), flush=True)
     res["qkv_gemm_bias_cost"] = bias_gemm_cost(iters=50, rounds=6)
+    res["qkv_gemm_qk_norm_cost"] = qk_norm_cost(iters=50, rounds=6)
     res["card_after"] = card()
     print(json.dumps(res, indent=1))
     if a.out:
