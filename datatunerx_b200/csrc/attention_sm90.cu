@@ -158,6 +158,20 @@ __device__ __forceinline__ void rope_inverse_frag(float (&o)[64], const float2* 
       }
 }
 
+// GLM's inverse rotary (partial, interleaved) on a 64 x 128 fragment: columns 2i, 2i + 1 (i < 32) are o[4 * j + 2 * hr + 0 / 1]
+// with i = 4 * j + cq / 2, from the transposed [32][stride] table; columns 64..127 pass through
+__device__ __forceinline__ void rope_glm_inverse_frag(float (&o)[64], const float2* cs, int stride, int pos0, int cq) {
+#pragma unroll
+  for (int j = 0; j < 8; ++j)
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      const float2 t = __ldg(cs + static_cast<size_t>(4 * j + (cq >> 1)) * stride + pos0 + 8 * hr);
+      const float x0 = o[4 * j + 2 * hr], x1 = o[4 * j + 2 * hr + 1];
+      o[4 * j + 2 * hr] = x0 * t.x + x1 * t.y;
+      o[4 * j + 2 * hr + 1] = x1 * t.x - x0 * t.y;
+    }
+}
+
 // 64 x 128 fragment * mul -> bf16 -> 128B-swizzled staging tile (two 64-column subtiles `sub` bytes apart at `stage`; this
 // thread's rows are row0 and row0 + 8 of the tile, the warpgroup's 64 rows start at wg_row0) -> two [64 x 64] TMA stores at
 // (grow, gcol) / (grow, gcol + 64) by one thread of the warpgroup (named barrier `bar_id`)
@@ -351,7 +365,8 @@ constexpr int DQ_XD = DQ_BAR + 256;            // [128] delta of the tile's rows
 constexpr int DQ_SMEM = DQ_XD + 512 + 1024;
 
 // WIN: see attn_fwd_kernel.  EXP_FMA: every N-th pair of exponentials on the FMA pipe (A/B switch "attn_dq_exp_fma_every").
-template <bool WIN, int EXP_FMA>
+// GLM: the inverse rotary of dQ is GLM's (rope_glm_inverse_frag, [32][rope_stride] table).
+template <bool WIN, int EXP_FMA, bool GLM = false>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 attn_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
                const __grid_constant__ CUtensorMap tmDO, const __grid_constant__ CUtensorMap tmO,
@@ -498,7 +513,10 @@ attn_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
     wgmma_touch(dq);
     if (lane == 0) mbar_arrive(&bar_free[slot]);
   }
-  if (p.rope_cs) rope_inverse_frag(dq, p.rope_cs, p.rope_stride, q0 + r0, cq);
+  if (p.rope_cs) {
+    if (GLM) rope_glm_inverse_frag(dq, p.rope_cs, p.rope_stride, q0 + r0, cq);
+    else rope_inverse_frag(dq, p.rope_cs, p.rope_stride, q0 + r0, cq);
+  }
   // dQ tile -> bf16 -> staging tile (this warpgroup's rows of the Q landing zone) -> TMA store
   store_frag_tma(dq, 1.f, 1.f, smem + DQ_SQ, 16384, r0, cq, cw * 64, &tmOut, colQ, row_base + qw0, 1 + cw, (tid & 127) == 0);
 }
@@ -515,7 +533,7 @@ constexpr int DKV_STAT = DKV_SDO + DKV_NS * 16384;  // DKV_NS x (lse2[64], delta
 constexpr int DKV_BAR = DKV_STAT + DKV_NS * 512;
 constexpr int DKV_SMEM = DKV_BAR + 256 + 1024;
 
-template <bool WIN>
+template <bool WIN, bool GLM = false>  // GLM: see attn_dq_kernel
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 attn_dkv_kernel(const __grid_constant__ CUtensorMap tmKV128, const __grid_constant__ CUtensorMap tmQ64,
                 const __grid_constant__ CUtensorMap tmDO64, const __grid_constant__ CUtensorMap tmOut, const AttnKParams p) {
@@ -653,7 +671,10 @@ attn_dkv_kernel(const __grid_constant__ CUtensorMap tmKV128, const __grid_consta
   }
   // dV, dK (with the inverse rotary) -> bf16 -> staging tiles (this warpgroup's rows of the V / K tiles) -> TMA stores
   store_frag_tma(dv, 1.f, 1.f, smem + DKV_SV, 16384, r0, cq, cw * 64, &tmOut, colV, row_base + kw0, 1 + cw, (tid & 127) == 0);
-  if (p.rope_cs) rope_inverse_frag(dk, p.rope_cs, p.rope_stride, kv0 + r0, cq);
+  if (p.rope_cs) {
+    if (GLM) rope_glm_inverse_frag(dk, p.rope_cs, p.rope_stride, kv0 + r0, cq);
+    else rope_inverse_frag(dk, p.rope_cs, p.rope_stride, kv0 + r0, cq);
+  }
   store_frag_tma(dk, 1.f, 1.f, smem + DKV_SK, 16384, r0, cq, cw * 64, &tmOut, colK, row_base + kw0, 1 + cw, (tid & 127) == 0);
 }
 
@@ -694,6 +715,11 @@ cudaError_t attn_init_device() {
     if ((e = set_smem(f, DQ_SMEM)) != cudaSuccess) return e;
   if ((e = set_smem(reinterpret_cast<const void*>(attn_dkv_kernel<false>), DKV_SMEM)) != cudaSuccess) return e;
   if ((e = set_smem(reinterpret_cast<const void*>(attn_dkv_kernel<true>), DKV_SMEM)) != cudaSuccess) return e;
+  const void* glm[] = {reinterpret_cast<const void*>(attn_dq_kernel<false, 0, true>), reinterpret_cast<const void*>(attn_dq_kernel<false, 3, true>),
+                       reinterpret_cast<const void*>(attn_dq_kernel<false, 4, true>)};
+  for (const void* f : glm)
+    if ((e = set_smem(f, DQ_SMEM)) != cudaSuccess) return e;
+  if ((e = set_smem(reinterpret_cast<const void*>(attn_dkv_kernel<false, true>), DKV_SMEM)) != cudaSuccess) return e;
   if (dev >= 0 && dev < 64) done[dev] = true;
   return cudaSuccess;
 }
@@ -740,6 +766,8 @@ cudaError_t attn_fwd(const AttnArgs& a, cudaStream_t s) {
 cudaError_t attn_bwd(const AttnArgs& a, cudaStream_t s) {
   if (a.S % 128 || a.B <= 0 || a.H <= 0 || !a.delta || !a.lse || !a.dout || !a.dqkv) return cudaErrorInvalidValue;
   if (a.window < 0) return cudaErrorInvalidValue;
+  // GLM's inverse rotary is instantiated for plain causal attention (GLM has no sliding window)
+  if (a.rope_glm != 0 && (a.rope_glm != 1 || a.window > 0)) return cudaErrorInvalidValue;
   cudaError_t e = attn_init_device();
   if (e != cudaSuccess) return e;
   const int Hkv = a.Hkv > 0 ? a.Hkv : a.H;
@@ -770,6 +798,13 @@ cudaError_t attn_bwd(const AttnArgs& a, cudaStream_t s) {
   p.row_start = a.row_start;
   const int gq = a.B * a.H * (a.S / 128), gkv = a.B * Hkv * (a.S / 128);
   const bool win = a.window > 0;
+  if (a.rope_glm && a.rope_cs) {
+#define DTX_DQ_GLM_LAUNCH(I) attn_dq_kernel<false, I, true><<<gq, ATT_THREADS, DQ_SMEM, s>>>(tmQ128, tmKV64, tmDO128, tmO128, tmDqkv64, p)
+    if (g_dq_exp_fma_every == 3) DTX_DQ_GLM_LAUNCH(3); else if (g_dq_exp_fma_every == 4) DTX_DQ_GLM_LAUNCH(4); else DTX_DQ_GLM_LAUNCH(0);
+#undef DTX_DQ_GLM_LAUNCH
+    attn_dkv_kernel<false, true><<<gkv, ATT_THREADS, DKV_SMEM, s>>>(tmQ128, tmKV64, tmDO64, tmDqkv64, p);
+    return cudaGetLastError();
+  }
 #define DTX_DQ_LAUNCH(W, I) attn_dq_kernel<W, I><<<gq, ATT_THREADS, DQ_SMEM, s>>>(tmQ128, tmKV64, tmDO128, tmO128, tmDqkv64, p)
   if (win) { if (g_dq_exp_fma_every == 3) DTX_DQ_LAUNCH(true, 3); else if (g_dq_exp_fma_every == 4) DTX_DQ_LAUNCH(true, 4); else DTX_DQ_LAUNCH(true, 0); }
   else { if (g_dq_exp_fma_every == 3) DTX_DQ_LAUNCH(false, 3); else if (g_dq_exp_fma_every == 4) DTX_DQ_LAUNCH(false, 4); else DTX_DQ_LAUNCH(false, 0); }

@@ -92,6 +92,31 @@ int32_t dtx_qk_norm_bwd(void* dy, int64_t ld, const void* x, int64_t ldx, int32_
                         S(stream)));
 }
 
+int32_t dtx_gemm_rope_glm(const void* A, int64_t lda, const void* B, int64_t ldb, int32_t b_mn, const void* A2, int64_t lda2,
+                          const void* B2, int64_t ldb2, int32_t K2, void* C, int64_t ldc, const void* rope_cs, int32_t rope_S,
+                          int32_t rope_cols, const void* rope_pos, int32_t M, int32_t N, int32_t K, const void* bias, void* stream) {
+  GemmArgs g;
+  g.A = static_cast<const bf16*>(A); g.lda = lda;
+  g.B = static_cast<const bf16*>(B); g.ldb = ldb; g.b_mn_major = b_mn;
+  g.A2 = static_cast<const bf16*>(A2); g.lda2 = lda2; g.B2 = static_cast<const bf16*>(B2); g.ldb2 = ldb2; g.K2 = K2;
+  g.C = C; g.ldc = ldc;
+  g.rope_cs = static_cast<const float2*>(rope_cs); g.rope_S = rope_S; g.rope_cols = rope_cols;
+  g.rope_pos = static_cast<const int32_t*>(rope_pos); g.rope_glm = 1;
+  g.M = M; g.N = N; g.K = K; g.epilogue = EPI_ROPE; g.bias = static_cast<const bf16*>(bias);
+  return rc(gemm_bf16(g, S(stream)));
+}
+
+int32_t dtx_rope_glm_qk(void* qkv, const void* cs, int32_t B, int32_t Sq, int32_t H, int32_t Hkv, int32_t inverse, void* stream) {
+  return rc(rope_glm_qk_inplace(static_cast<bf16*>(qkv), static_cast<const float2*>(cs), B, Sq, H + Hkv, (H + 2 * Hkv) * 128, inverse,
+                                S(stream)));
+}
+
+int32_t dtx_post_norm_add(const void* y, const void* w, const void* res, void* out, void* rstd, int32_t M, int32_t d, float eps,
+                          void* stream) {
+  return rc(post_norm_add(static_cast<const bf16*>(y), static_cast<const bf16*>(w), static_cast<const bf16*>(res), static_cast<bf16*>(out),
+                          static_cast<float*>(rstd), M, d, eps, S(stream)));
+}
+
 int32_t dtx_set_option(const char* name, int32_t value) {
   if (!name) return DTX_ERR_INVALID;
   if (strcmp(name, "gemm_pair_kernel") == 0) {
@@ -225,7 +250,13 @@ int32_t dtx_attn_fwd(const void* qkv, void* out, void* lse2, int32_t B, int32_t 
 int32_t dtx_attn_bwd(const void* qkv, const void* out, const void* dout, const void* lse2, void* delta, void* dqkv, int32_t B,
                      int32_t Sq, int32_t H, int32_t Hkv, float scale, const void* seq_lens, int32_t window, const void* rope_cs_t,
                      int32_t rope_stride, void* stream) {
+  return dtx_attn_bwd_rope(qkv, out, dout, lse2, delta, dqkv, B, Sq, H, Hkv, scale, seq_lens, window, rope_cs_t, rope_stride, 0, stream);
+}
+int32_t dtx_attn_bwd_rope(const void* qkv, const void* out, const void* dout, const void* lse2, void* delta, void* dqkv, int32_t B,
+                          int32_t Sq, int32_t H, int32_t Hkv, float scale, const void* seq_lens, int32_t window, const void* rope_cs_t,
+                          int32_t rope_stride, int32_t rope_glm, void* stream) {
   AttnArgs a;
+  a.rope_glm = rope_glm;
   a.Hkv = Hkv;
   a.qkv = static_cast<const bf16*>(qkv); a.out = const_cast<bf16*>(static_cast<const bf16*>(out));
   a.lse = const_cast<float*>(static_cast<const float*>(lse2)); a.dout = static_cast<const bf16*>(dout);

@@ -112,6 +112,55 @@ __global__ void __launch_bounds__(RMS_THREADS) rmsnorm_fwd_kernel(const bf16* __
   }
 }
 
+// Glm4's post-sublayer norm and the residual add in one pass: out = res + w * (y * rsqrt(mean(y^2) + eps)), rstd saved (its
+// backward is rmsnorm_bwd on y with dres = null).  out may be null: rstd only (the per-layer recompute refills it).
+template <int NCH>
+__global__ void __launch_bounds__(RMS_THREADS) post_norm_add_kernel(const bf16* __restrict__ y, const bf16* __restrict__ w,
+                                                                    const bf16* __restrict__ res, bf16* __restrict__ out,
+                                                                    float* __restrict__ rstd, int d, float eps) {
+  __shared__ float sh[4];
+  const size_t off = static_cast<size_t>(blockIdx.x) * d;
+  const uint4* yr = reinterpret_cast<const uint4*>(y + off);
+  const int nvec = d >> 3;
+  uint4 buf[NCH];
+  float ss = 0.f;
+#pragma unroll
+  for (int i = 0; i < NCH; ++i) {
+    const int v = i * RMS_THREADS + threadIdx.x;
+    if (v < nvec) buf[i] = ldg_stream(yr + v);
+  }
+#pragma unroll
+  for (int i = 0; i < NCH; ++i) {
+    const int v = i * RMS_THREADS + threadIdx.x;
+    if (v < nvec) {
+      float f[8];
+      bf16x8_to_f32(buf[i], f);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) ss += f[j] * f[j];
+    }
+  }
+  ss = block_sum_128(ss, sh);
+  const float r = rsqrtf(ss / static_cast<float>(d) + eps);
+  if (threadIdx.x == 0) rstd[blockIdx.x] = r;
+  if (!out) return;
+  const uint4* wr = reinterpret_cast<const uint4*>(w);
+  const uint4* rr = reinterpret_cast<const uint4*>(res + off);
+  uint4* orow = reinterpret_cast<uint4*>(out + off);
+#pragma unroll
+  for (int i = 0; i < NCH; ++i) {
+    const int v = i * RMS_THREADS + threadIdx.x;
+    if (v < nvec) {
+      float f[8], g[8], q[8];
+      bf16x8_to_f32(buf[i], f);
+      bf16x8_to_f32(__ldg(wr + v), g);
+      bf16x8_to_f32(ldg_stream(rr + v), q);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) f[j] = q[j] + f[j] * r * g[j];
+      orow[v] = f32_to_bf16x8(f);
+    }
+  }
+}
+
 // dx = rstd * (w*dy) - x * rstd^3 * mean(w*dy*x) (+ dres).  Base weights are frozen: no dw.
 template <int NCH>
 __global__ void __launch_bounds__(RMS_THREADS) rmsnorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x,
@@ -215,6 +264,34 @@ __global__ void rope_kernel(bf16* __restrict__ qkv, const float2* __restrict__ c
     }
     *reinterpret_cast<uint4*>(base) = f32_to_bf16x8(a);
     *reinterpret_cast<uint4*>(base + half) = f32_to_bf16x8(b);
+  }
+}
+
+// GLM's partial interleaved rotary (transformers modeling_glm apply_rotary_pos_emb), in place on q and k of packed qkv:
+//   out[2i] = x[2i] cos_i - x[2i+1] sin_i ; out[2i+1] = x[2i+1] cos_i + x[2i] sin_i  (i < 32); columns 64..127 of a head untouched.
+// One thread per 8 columns (four pairs, one uint4) of the rotated 64; cs table: [S][32] float2(cos, sin).
+__global__ void rope_glm_kernel(bf16* __restrict__ qkv, const float2* __restrict__ cs, int S, int NH, int W, int inverse,
+                                long long total_vec) {
+  for (long long t = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; t < total_vec;
+       t += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int iv = static_cast<int>(t & 7);
+    const long long r = t >> 3;
+    const int h = static_cast<int>(r % NH);
+    const long long m = r / NH;
+    const int pos = static_cast<int>(m % S);
+    uint4* base = reinterpret_cast<uint4*>(qkv + m * static_cast<long long>(W) + static_cast<long long>(h) * 128 + iv * 8);
+    float a[8];
+    bf16x8_to_f32(*base, a);
+    const float2* c = cs + static_cast<size_t>(pos) * 32 + iv * 4;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float2 v = __ldg(c + j);
+      const float sn = inverse ? -v.y : v.y;
+      const float x0 = a[2 * j], x1 = a[2 * j + 1];
+      a[2 * j] = x0 * v.x - x1 * sn;
+      a[2 * j + 1] = x1 * v.x + x0 * sn;
+    }
+    *base = f32_to_bf16x8(a);
   }
 }
 
@@ -962,6 +1039,18 @@ cudaError_t rmsnorm_fwd(const bf16* x, const bf16* w, bf16* y, float* rstd, int 
   return cudaGetLastError();
 }
 
+cudaError_t post_norm_add(const bf16* y, const bf16* w, const bf16* res, bf16* out, float* rstd, int M, int d, float eps,
+                          cudaStream_t s) {
+  if (d % 8 || d > 8192 || M < 0 || !rstd || (out && (!w || !res))) return cudaErrorInvalidValue;
+  if (M == 0) return cudaSuccess;
+  const int nch = (d / 8 + RMS_THREADS - 1) / RMS_THREADS;
+  if (nch <= 1) post_norm_add_kernel<1><<<M, RMS_THREADS, 0, s>>>(y, w, res, out, rstd, d, eps);
+  else if (nch <= 2) post_norm_add_kernel<2><<<M, RMS_THREADS, 0, s>>>(y, w, res, out, rstd, d, eps);
+  else if (nch <= 4) post_norm_add_kernel<4><<<M, RMS_THREADS, 0, s>>>(y, w, res, out, rstd, d, eps);
+  else post_norm_add_kernel<8><<<M, RMS_THREADS, 0, s>>>(y, w, res, out, rstd, d, eps);
+  return cudaGetLastError();
+}
+
 cudaError_t rmsnorm_bwd(const bf16* dy, const bf16* x, const bf16* w, const float* rstd, const bf16* dres, bf16* dx, int M,
                         int d, cudaStream_t s, const int32_t* row_map) {
   if (d % 8 || d > 8192) return cudaErrorInvalidValue;
@@ -978,6 +1067,13 @@ cudaError_t rope_qk_inplace_table(bf16* qkv, const float2* cs, int B, int S, int
   if (D % 16) return cudaErrorInvalidValue;
   const long long total = static_cast<long long>(B) * S * n_rot_heads * (D / 16);
   rope_kernel<<<grid_for(total, 256), 256, 0, s>>>(qkv, cs, S, n_rot_heads, W, D, inverse, total);
+  return cudaGetLastError();
+}
+
+cudaError_t rope_glm_qk_inplace(bf16* qkv, const float2* cs, int B, int S, int n_rot_heads, int W, int inverse, cudaStream_t s) {
+  if (W % 8 || n_rot_heads * 128 > W || B <= 0 || S <= 0) return cudaErrorInvalidValue;
+  const long long total = static_cast<long long>(B) * S * n_rot_heads * 8;
+  rope_glm_kernel<<<grid_for(total, 256), 256, 0, s>>>(qkv, cs, S, n_rot_heads, W, inverse, total);
   return cudaGetLastError();
 }
 

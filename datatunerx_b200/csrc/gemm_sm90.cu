@@ -84,7 +84,10 @@ __device__ __forceinline__ float round_bf16(float x) { return __bfloat162float(_
 // quad (32 each): 32 products and two shfl.xor give the sum of squares.  The pre-norm x is stored to tmX (aux [M, rope_cols])
 // in an extra pass before the normalised head goes to C.  The two weight vectors sit in the warpgroup's bias row (read with
 // ld.shared: with __ldg the compiler hoists the loads and the epilogue spills).
-template <int BN, bool A_MN, bool B_MN, int EPI, bool BIAS = false, bool QKNORM = false>
+// ROPE_GLM (EPI_ROPE only, without QKNORM): GLM's partial interleaved rotary - only columns 0..63 of every rotated head turn, in
+// adjacent pairs (2i, 2i + 1) with frequency i; columns 64..127 pass through.  A pair is two neighbouring accumulator registers of
+// one thread, so no shuffles are needed; the table is [S][32].
+template <int BN, bool A_MN, bool B_MN, int EPI, bool BIAS = false, bool QKNORM = false, bool ROPE_GLM = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
             const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
@@ -93,6 +96,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   static_assert(EPI < EPI_ROPE || BN == 256, "the fused epilogues pair columns 64 / 128 apart inside one 256-column tile");
   static_assert(!BIAS || EPI == EPI_BF16 || EPI == EPI_ROPE, "the bias is added by the EPI_BF16 and EPI_ROPE epilogues only");
   static_assert(!QKNORM || (EPI == EPI_ROPE && !BIAS), "the q/k norm runs in the EPI_ROPE epilogue, without a bias");
+  static_assert(!ROPE_GLM || (EPI == EPI_ROPE && !QKNORM), "the GLM rotary runs in the EPI_ROPE epilogue, without the q/k norm");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::RING_BYTES + Cfg::STG_BYTES);
@@ -326,14 +330,16 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
           pass_store(&tmC, p.c_cols, n0 + 64 * ps, 32, 2, y0, split);
         }
       } else if (EPI == EPI_ROPE) {
-        // two heads per tile (columns 0-127 / 128-255), one per pass; rotary pairs column i with i + 64 of a head
+        // two heads per tile (columns 0-127 / 128-255), one per pass; rotary pairs column i with i + 64 of a head (ROPE_GLM:
+        // column 2i with 2i + 1 of the first 64)
         const bool rot = n0 < p.rope_cols;
         const float2* cs[2];
 #pragma unroll
         for (int hr = 0; hr < 2; ++hr) {
           const int row = y0 + wq * 16 + rq + 8 * hr;
           const int pos = row >= p.M ? 0 : (p.rope_pos ? __ldg(p.rope_pos + row) : row % p.rope_S);
-          cs[hr] = p.rope_cs + static_cast<long long>(pos) * 64;
+          if constexpr (ROPE_GLM) cs[hr] = p.rope_cs + static_cast<long long>(pos) * 32;
+          else cs[hr] = p.rope_cs + static_cast<long long>(pos) * 64;
         }
 #pragma unroll
         for (int hh = 0; hh < 2; ++hh) {
@@ -390,7 +396,15 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
                 hi[0] += bh.x;
                 hi[1] += bh.y;
               }
-              if (rot) {
+              if constexpr (ROPE_GLM) {
+                if (rot) {  // columns 8 jj + cq, + 1 of the head are pair 4 jj + cq / 2
+                  const float2 t = __ldg(cs[hr] + jj * 4 + (cq >> 1));
+                  const float sn = p.rope_inverse ? -t.y : t.y;
+                  const float x0 = lo[0], x1 = lo[1];
+                  lo[0] = x0 * t.x - x1 * sn;
+                  lo[1] = x1 * t.x + x0 * sn;
+                }
+              } else if (rot) {
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
                   const float2 t = __ldg(cs[hr] + jj * 8 + cq + e);
@@ -557,11 +571,11 @@ struct DeviceOnce {
 int g_wide_tiles = 1;
 int g_group_m = GROUP_M;
 
-template <int BN, bool A_MN, bool B_MN, int EPI, bool BIAS = false, bool QKNORM = false>
+template <int BN, bool A_MN, bool B_MN, int EPI, bool BIAS = false, bool QKNORM = false, bool ROPE_GLM = false>
 cudaError_t launch(const GemmArgs& a, cudaStream_t s) {
   using Cfg = GemmCfg<BN>;
   constexpr int SMEM = Cfg::SMEM_BYTES + (BIAS || QKNORM ? Cfg::BIAS_BYTES : 0);
-  auto kern = gemm_kernel<BN, A_MN, B_MN, EPI, BIAS, QKNORM>;
+  auto kern = gemm_kernel<BN, A_MN, B_MN, EPI, BIAS, QKNORM, ROPE_GLM>;
   static DeviceOnce attr;  // the attribute is per device: a second trainer on another GPU of the same process needs it too
   if (cudaError_t e = attr.run([&] { return cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM); });
       e != cudaSuccess)
@@ -657,6 +671,9 @@ cudaError_t launch_epi(const GemmArgs& a, cudaStream_t s) {
 
 template <bool B_MN>
 cudaError_t launch_fused(const GemmArgs& a, cudaStream_t s) {
+  if (a.rope_glm) {  // EPI_ROPE without the q/k norm (checked by gemm_bf16)
+    return a.bias ? launch<256, false, B_MN, EPI_ROPE, true, false, true>(a, s) : launch<256, false, B_MN, EPI_ROPE, false, false, true>(a, s);
+  }
   if (a.bias) return a.epilogue == EPI_ROPE ? launch<256, false, B_MN, EPI_ROPE, true>(a, s) : cudaErrorInvalidValue;
   if (a.qk_wq) return a.epilogue == EPI_ROPE ? launch<256, false, B_MN, EPI_ROPE, false, true>(a, s) : cudaErrorInvalidValue;
   switch (a.epilogue) {
@@ -695,6 +712,8 @@ cudaError_t gemm_bf16(const GemmArgs& a, cudaStream_t s) {
                   (reinterpret_cast<uintptr_t>(a.aux) & 15) || (reinterpret_cast<uintptr_t>(a.qk_wq) & 3) ||
                   (reinterpret_cast<uintptr_t>(a.qk_wk) & 3)))
     return cudaErrorInvalidValue;
+  // GLM rotary: EPI_ROPE only, not combined with the q/k norm
+  if (a.rope_glm && (a.rope_glm != 1 || a.epilogue != EPI_ROPE || a.qk_wq)) return cudaErrorInvalidValue;
   // TMA needs 16-byte aligned bases and row strides
   if ((a.lda & 7) || (a.ldb & 7) || (reinterpret_cast<uintptr_t>(a.A) & 15) || (reinterpret_cast<uintptr_t>(a.B) & 15))
     return cudaErrorInvalidValue;

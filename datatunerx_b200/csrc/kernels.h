@@ -43,6 +43,9 @@ struct GemmArgs {
   const bf16 *qk_wq = nullptr, *qk_wk = nullptr;
   int qk_q_cols = 0;
   float qk_eps = 0.f;
+  // 1 (EPI_ROPE only, no q/k norm): GLM's partial interleaved rotary instead of the half-split one - columns 2i, 2i + 1 of the
+  // first 64 of every rotated head turn by frequency i, columns 64..127 pass through; rope_cs is then [S][32]
+  int rope_glm = 0;
   int M = 0, N = 0, K = 0;
   // optional device-side row count (<= M): 256-row blocks of tiles that start at or beyond it are skipped (rows up to the
   // end of the last live block are still computed).  Lets the lm_head GEMMs run over the unmasked tokens only without a
@@ -96,6 +99,7 @@ struct AttnArgs {
   // backward
   int rope_stride = 0;              // row stride (positions) of the transposed rope table; 0 = S
   const float2* rope_cs = nullptr;  // backward only: TRANSPOSED table [64][S] (cos, sin); if set, dq and dk get the inverse rotary applied before the store
+  int rope_glm = 0;                 // 1: that inverse rotary is GLM's (partial, interleaved; table [32][S]); needs window 0
   const bf16* dout = nullptr;  // [B*S, H*D]
   bf16* dqkv = nullptr;        // [B*S, (H + 2*Hkv)*D]
   float* delta = nullptr;      // [B, H, S] scratch: rowsum(dO * O)
@@ -115,10 +119,17 @@ cudaError_t rmsnorm_fwd(const bf16* x, const bf16* w, bf16* y, float* rstd, int 
 // row_map (optional, [M]): the gradient of row m sits in row row_map[m] of dy; rows with row_map[m] < 0 get dx = dres (or 0).
 cudaError_t rmsnorm_bwd(const bf16* dy, const bf16* x, const bf16* w, const float* rstd, const bf16* dres, bf16* dx,
                         int M, int d, cudaStream_t s, const int32_t* row_map = nullptr);
+// Glm4 post-sublayer norm + residual add: out = res + w * (y * rsqrt(mean(y^2) + eps)) (fp32, one block per row), rstd[M] saved
+// for rmsnorm_bwd(dy, y, w, rstd, dres = null).  out = null computes rstd only.
+cudaError_t post_norm_add(const bf16* y, const bf16* w, const bf16* res, bf16* out, float* rstd, int M, int d, float eps,
+                          cudaStream_t s);
 // half-split rotary embedding applied in place to the first n_rot_heads heads (q heads then k heads) of every row of
 // packed qkv (row stride W elements). inverse=1 applies R^T (backward).  cs = [S][D/2] float2(cos, sin) table
 cudaError_t rope_qk_inplace_table(bf16* qkv, const float2* cs, int B, int S, int n_rot_heads, int W, int D, int inverse,
                                   cudaStream_t s);
+// GLM's partial interleaved rotary, the same way: columns 2i, 2i + 1 (i < 32) of every one of the first n_rot_heads 128-column heads
+// turn by cs[pos][i] (cs = [S][32]), columns 64..127 are left as they are
+cudaError_t rope_glm_qk_inplace(bf16* qkv, const float2* cs, int B, int S, int n_rot_heads, int W, int inverse, cudaStream_t s);
 // gu [M, 2F]: [gate F | up F] (interleaved = 0) or the GU-interleaved layout the trainer uses (interleaved = 1: feature f
 // has its gate at column (f/128)*256 + f%128 and its up 128 columns further); act[M,F] = silu(gate) * up
 cudaError_t swiglu_fwd(const bf16* gu, bf16* act, int M, int F, int interleaved, cudaStream_t s);

@@ -151,6 +151,10 @@ struct Layer {
   bf16* bias = nullptr;  // dtx_model_ext.qkv_bias: [W] q|k|v biases in the row order of wqkv (bf16 also under NF4), else null
   bf16* qkn = nullptr;   // dtx_model_ext.qk_norm: [2 * 128] q_norm | k_norm weights (bf16 also under NF4), else null
   bf16* qk_pre = nullptr;  // qk_norm, saved: [M, dq + dkv] q|k projection output before the norm (bf16)
+  bf16* pn = nullptr;  // dtx_model_ext.post_norms: [2 * d] post_self_attn_layernorm | post_mlp_layernorm (bf16 also under NF4)
+  // post_norms, saved: the o- and down-projection outputs before their norms [M, d] and the norms' rstd [M]
+  bf16 *o_pre = nullptr, *down_pre = nullptr;
+  float *rstd_pn1 = nullptr, *rstd_pn2 = nullptr;
   bf16 *a_cat = nullptr, *b_ext = nullptr;                                               // shadows
   bf16 *h1 = nullptr, *t = nullptr, *qkv = nullptr, *attn = nullptr, *x_mid = nullptr, *gu = nullptr;  // saved
   bf16* hd = nullptr;  // LoRA dropout only: [M, nt*d] dropped copies of h1, one per target (peft: one nn.Dropout per module)
@@ -243,6 +247,9 @@ struct dtx_trainer {
   bool qkv_bias = false;        // q|k|v biases (Qwen2): Layer::bias; full-parameter SFT keeps them at off_bias of the layer block
   int64_t off_bias = 0;
   bool qk_norm = false;         // q/k RMSNorm (Qwen3): Layer::qkn, Layer::qk_pre; full-parameter SFT keeps the weights at off_qkn
+  bool rope_glm = false;        // GLM's partial interleaved rotary: rope_cs / rope_cs_t hold head_dim / 4 frequencies
+  bool post_norms = false;      // Glm4's post-sublayer norms: Layer::pn, o_pre, down_pre; full-parameter SFT keeps pn at off_pn
+  int64_t off_pn = 0;
   int64_t off_qkn = 0;
   int64_t layer_elems = 0, glob_elems = 0;
   int64_t off_wo = 0, off_wgu = 0, off_wdown = 0, off_n1 = 0, off_n2 = 0, goff_lm = 0, goff_nf = 0, layer_used = 0, glob_used = 0;
@@ -272,6 +279,7 @@ struct dtx_trainer {
   std::vector<uint8_t> loaded;
   std::vector<uint8_t> bias_loaded;  // qkv_bias: q, k, v bias of every layer
   std::vector<uint8_t> qkn_loaded;   // qk_norm: q_norm, k_norm weight of every layer
+  std::vector<uint8_t> pn_loaded;    // post_norms: post_self_attn_layernorm, post_mlp_layernorm weight of every layer
   bool all_random = false;
   bool have_lora = false;
   cudaEvent_t ev_fb = nullptr, ev_ar = nullptr;
@@ -348,6 +356,11 @@ struct dtx_trainer {
         snprintf(buf, n, "model.layers.%zu.self_attn.%s.weight", i / 2, i % 2 ? "k_norm" : "q_norm");
         return buf;
       }
+    for (size_t i = 0; i < pn_loaded.size(); ++i)
+      if (!pn_loaded[i]) {
+        snprintf(buf, n, "model.layers.%zu.%s.weight", i / 2, i % 2 ? "post_mlp_layernorm" : "post_self_attn_layernorm");
+        return buf;
+      }
     return nullptr;
   }
 };
@@ -404,10 +417,12 @@ int pick_split(int n_sms, int m_tiles, int kb_total) {
 // (_compute_linear_scaling_rope_parameters), llama3 follows _compute_llama3_parameters - wavelen = 2 pi / inv_freq (torch
 // evaluates a scalar over a tensor as reciprocal times scalar), wavelengths below original_max_pos / high_freq_factor keep their
 // frequency, those above original_max_pos / low_freq_factor are divided by the factor, the band between is interpolated.
+// GLM (ext.rope_glm) rotates the first rotary_dim = head_dim / 2 dims only: GlmRotaryEmbedding builds theta^(-2i/rotary_dim).
+int rope_rotary_dim(const dtx_model_cfg& mc, const dtx_model_ext& ext) { return ext.rope_glm ? mc.head_dim / 2 : mc.head_dim; }
 void rope_inv_freq(const dtx_model_cfg& mc, const dtx_model_ext& ext, float* out) {
-  const int half = mc.head_dim / 2;
+  const int rd = rope_rotary_dim(mc, ext), half = rd / 2;
   for (int i = 0; i < half; ++i) {
-    const float base = 1.0f / powf(mc.rope_theta, static_cast<float>(2 * i) / static_cast<float>(mc.head_dim));
+    const float base = 1.0f / powf(mc.rope_theta, static_cast<float>(2 * i) / static_cast<float>(rd));
     float f = base;
     if (ext.rope_type == DTX_ROPE_LINEAR) {
       f = base / ext.rope_factor;
@@ -457,6 +472,10 @@ int create_buffers(dtx_trainer* t) {
       t->off_qkn = t->layer_used;
       t->layer_used += NQK;
     }
+    if (t->post_norms) {  // and for the post-sublayer norm weights ("layernorm" names)
+      t->off_pn = t->layer_used;
+      t->layer_used += 2 * d;
+    }
     t->layer_elems = pad(t->layer_used);
     t->goff_lm = V * d;
     t->goff_nf = 2 * V * d;
@@ -487,6 +506,7 @@ int create_buffers(dtx_trainer* t) {
   t->loaded.assign(3 + 9 * L, 0);
   t->bias_loaded.assign(t->qkv_bias ? 3 * L : 0, 0);
   t->qkn_loaded.assign(t->qk_norm ? 2 * L : 0, 0);
+  t->pn_loaded.assign(t->post_norms ? 2 * L : 0, 0);
   t->layers.resize(L);
   t->xs.resize(L + 1);
   for (size_t l = 0; l <= L; ++l) ok = ok && t->alloc(&t->xs[l], M * d);
@@ -498,20 +518,24 @@ int create_buffers(dtx_trainer* t) {
       y.norm1 = blk + t->off_n1; y.norm2 = blk + t->off_n2;
       if (t->qkv_bias) y.bias = blk + t->off_bias;
       if (t->qk_norm) y.qkn = blk + t->off_qkn;
+      if (t->post_norms) y.pn = blk + t->off_pn;
     } else {
       ok = ok && t->alloc(&y.wqkv, W * d) && t->alloc(&y.wo, d * dq) && t->alloc(&y.wgu, 2 * F * d) &&
            t->alloc(&y.wdown, d * F) && t->alloc(&y.norm1, d) && t->alloc(&y.norm2, d);
       if (t->qkv_bias) ok = ok && t->alloc(&y.bias, W);
       if (t->qk_norm) ok = ok && t->alloc(&y.qkn, NQK);
+      if (t->post_norms) ok = ok && t->alloc(&y.pn, 2 * d);
       y.a_cat = t->a_cat_all + l * RP * KA;
       y.b_ext = t->b_ext_all + l * W * RP;
     }
     t->base_bytes +=
-        static_cast<int64_t>((W * d + d * dq + 3 * F * d + 2 * d + (t->qkv_bias ? W : 0) + (t->qk_norm ? NQK : 0)) * sizeof(bf16));
+        static_cast<int64_t>((W * d + d * dq + 3 * F * d + 2 * d + (t->qkv_bias ? W : 0) + (t->qk_norm ? NQK : 0) +
+                              (t->post_norms ? 2 * d : 0)) * sizeof(bf16));
     if (t->recompute == RECOMPUTE_LAYER && l > 0) {  // one saved set, refilled layer by layer
       const Layer& y0 = t->layers[0];
       y.h1 = y0.h1; y.t = y0.t; y.hd = y0.hd; y.qkv = y0.qkv; y.attn = y0.attn; y.x_mid = y0.x_mid; y.gu = y0.gu;
       y.qk_pre = y0.qk_pre;
+      y.o_pre = y0.o_pre; y.down_pre = y0.down_pre; y.rstd_pn1 = y0.rstd_pn1; y.rstd_pn2 = y0.rstd_pn2;
       y.lse = y0.lse; y.rstd1 = y0.rstd1; y.rstd2 = y0.rstd2;
       continue;
     }
@@ -519,6 +543,8 @@ int create_buffers(dtx_trainer* t) {
     ok = ok && t->alloc(&y.h1, M * d) && t->alloc(&y.qkv, M * W) &&
          t->alloc(&y.attn, M * dq) && t->alloc(&y.x_mid, M * d) && t->alloc(&y.gu, M * 2 * F);
     if (t->qk_norm) ok = ok && t->alloc(&y.qk_pre, M * QK);
+    if (t->post_norms)
+      ok = ok && t->alloc(&y.o_pre, M * d) && t->alloc(&y.down_pre, M * d) && t->alloc(&y.rstd_pn1, M) && t->alloc(&y.rstd_pn2, M);
     if (t->dropout) ok = ok && t->alloc(&y.hd, M * KA);
     ok = ok && t->alloc(&y.lse, static_cast<size_t>(tc.micro_batch) * mc.n_heads * tc.seq_len) && t->alloc(&y.rstd1, M) &&
          t->alloc(&y.rstd2, M);
@@ -552,13 +578,14 @@ int create_buffers(dtx_trainer* t) {
        t->alloc(&t->d_pos, M) && t->alloc(&t->d_row_start, static_cast<size_t>(tc.micro_batch) + 1);
   ok = ok && t->alloc(&t->d_seq_lens, static_cast<size_t>(tc.micro_batch)) && t->alloc(&t->d_row_sum, static_cast<size_t>(tc.micro_batch)) &&
        t->alloc(&t->d_row_valid, static_cast<size_t>(tc.micro_batch)) && t->alloc(&t->d_host_red, 64);
-  ok = ok && t->alloc(&t->rope_cs, static_cast<size_t>(tc.seq_len) * (mc.head_dim / 2));
-  ok = ok && t->alloc(&t->rope_cs_t, static_cast<size_t>(tc.seq_len) * (mc.head_dim / 2));
+  const int rope_half = rope_rotary_dim(mc, t->ext) / 2;
+  ok = ok && t->alloc(&t->rope_cs, static_cast<size_t>(tc.seq_len) * rope_half);
+  ok = ok && t->alloc(&t->rope_cs_t, static_cast<size_t>(tc.seq_len) * rope_half);
   if (!ok) return DTX_ERR_CUDA;
   if (t->dry) return DTX_OK;
   // rotary table in double precision (HF LlamaRotaryEmbedding; inverse frequencies of the model's rope type)
   {
-    const int half = mc.head_dim / 2;
+    const int half = rope_half;
     std::vector<float> inv_freq(half);
     rope_inv_freq(mc, t->ext, inv_freq.data());
     std::vector<float2> cs(static_cast<size_t>(tc.seq_len) * half);
@@ -758,12 +785,14 @@ int layer_fwd(dtx_trainer* t, int l, int phase, bool backward) {
       if (qk_wq) {  // q/k norm (Qwen3) before the rotary; the pre-norm q|k is saved for the backward pass
         g.qk_wq = qk_wq; g.qk_wk = qk_wk; g.qk_q_cols = dq; g.qk_eps = mc.rms_eps; g.aux = y.qk_pre; g.ld_aux = QK;
       }
+      g.rope_glm = t->rope_glm ? 1 : 0;
     }
     CK(gemm_bf16(g, s), 1);
   }
   if (!fused && t->packed) return t->fail(DTX_ERR_STATE, "packed batches need the fused RoPE epilogue");
   if (!fused && qk_wq) CK(qk_norm_fwd(y.qkv, W, M, dq, QK, qk_wq, qk_wk, mc.rms_eps, y.qk_pre, QK, s), 1);
-  if (!fused) CK(rope_qk_inplace_table(y.qkv, t->rope_cs, B, S, H + Hkv, W, D, 0, s), 1);
+  if (!fused && t->rope_glm) CK(rope_glm_qk_inplace(y.qkv, t->rope_cs, B, S, H + Hkv, W, 0, s), 1);
+  else if (!fused) CK(rope_qk_inplace_table(y.qkv, t->rope_cs, B, S, H + Hkv, W, D, 0, s), 1);
   {
     AttnArgs a;
     a.qkv = y.qkv; a.out = y.attn; a.lse = y.lse; a.B = B; a.S = S; a.H = H; a.Hkv = Hkv; a.scale = att_scale;
@@ -771,13 +800,15 @@ int layer_fwd(dtx_trainer* t, int l, int phase, bool backward) {
     if (t->packed) { a.row_start = t->d_row_start; a.total_rows = M; }
     CK(attn_fwd(a, s), 1);
   }
-  {  // x_mid = x + attn * Wo^T
+  {  // x_mid = x + attn * Wo^T   (post_norms: x_mid = x + post_self_attn_layernorm(o_pre), o_pre = attn * Wo^T)
     BASEW(W_O, wo);
     GemmArgs g;
     g.A = y.attn; g.lda = dq; g.B = wo; g.ldb = dq; g.C = y.x_mid; g.ldc = d; g.R = t->xs[l]; g.ldr = d;
     g.M = M; g.N = d; g.K = dq; g.epilogue = EPI_BF16_ADD;
+    if (y.pn) { g.C = y.o_pre; g.R = nullptr; g.ldr = 0; g.epilogue = EPI_BF16; }
     CK(gemm_bf16(g, s), 1);
   }
+  if (y.pn) CK(post_norm_add(y.o_pre, y.pn, t->xs[l], y.x_mid, y.rstd_pn1, M, d, mc.rms_eps, s), 1);
   CK(rmsnorm_fwd(y.x_mid, y.norm2, t->h2, y.rstd2, M, d, mc.rms_eps, s), 1);
   {  // [gate | up] = h2 * Wgu^T
     BASEW(W_GU, wgu);
@@ -790,13 +821,18 @@ int layer_fwd(dtx_trainer* t, int l, int phase, bool backward) {
     CK(gemm_bf16(g, s), 1);
   }
   if (!fused) CK(swiglu_fwd(y.gu, t->act, M, F, 1, s), 1);
-  if (phase == PH_FWD) {  // x_next = x_mid + act * Wdown^T
+  // x_next = x_mid + act * Wdown^T   (post_norms: x_next = x_mid + post_mlp_layernorm(down_pre), down_pre = act * Wdown^T; the
+  // recompute refills down_pre and its rstd, which the backward pass needs, and leaves the kept x_next alone)
+  if (phase == PH_FWD || y.pn) {
     BASEW(W_DOWN, wdown);
     GemmArgs g;
     g.A = t->act; g.lda = F; g.B = wdown; g.ldb = F; g.C = t->xs[l + 1]; g.ldc = d; g.R = y.x_mid; g.ldr = d;
     g.M = M; g.N = d; g.K = F; g.epilogue = EPI_BF16_ADD;
+    if (y.pn) { g.C = y.down_pre; g.R = nullptr; g.ldr = 0; g.epilogue = EPI_BF16; }
     CK(gemm_bf16(g, s), 1);
   }
+  if (y.pn)
+    CK(post_norm_add(y.down_pre, y.pn + d, y.x_mid, phase == PH_FWD ? t->xs[l + 1] : nullptr, y.rstd_pn2, M, d, mc.rms_eps, s), 1);
   return DTX_OK;
 }
 
@@ -884,14 +920,20 @@ int fwd_bwd(dtx_trainer* t, bool backward) {
     }
     Layer& y = t->layers[l];
     bf16* gl_w = t->full ? t->g_flat + static_cast<int64_t>(l) * t->layer_elems : nullptr;  // this layer's gradient block
+    const bf16* d_down = cur;  // gradient of the down-projection output
+    if (y.pn) {  // through post_mlp_layernorm: d down_pre into dh (free until the dh2 GEMM below); full SFT: its weight gradient
+      if (t->full) CK(rmsnorm_dw(cur, y.down_pre, y.rstd_pn2, M, d, t->ndw_scratch, gl_w + t->off_pn + d, accumulate, s), 2);
+      CK(rmsnorm_bwd(cur, y.down_pre, y.pn + d, y.rstd_pn2, nullptr, t->dh, M, d, s), 1);
+      d_down = t->dh;
+    }
     if (t->full) {  // dWdown = d x_out^T * act: act = silu(gate) * up is recomputed from the saved gate|up (one HBM-bound pass)
       CK(swiglu_fwd(y.gu, t->act, M, F, 1, s), 1);
-      CK(dw_gemm(cur, d, t->act, F, gl_w + t->off_wdown), 1);
+      CK(dw_gemm(d_down, d, t->act, F, gl_w + t->off_wdown), 1);
     }
     {  // dact = dx * Wdown ; fused: d[gate|up] straight from the accumulator, dact never touches HBM
       BASEW(W_DOWN, wdown);
       GemmArgs g;
-      g.A = cur; g.lda = d; g.B = wdown; g.ldb = F; g.b_mn_major = 1; g.C = t->dact; g.ldc = F;
+      g.A = d_down; g.lda = d; g.B = wdown; g.ldb = F; g.b_mn_major = 1; g.C = t->dact; g.ldc = F;
       g.M = M; g.N = F; g.K = d; g.epilogue = EPI_BF16;
       if (fused) {
         g.epilogue = EPI_SWIGLU_BWD; g.C = t->dgu; g.ldc = 2 * F; g.aux = y.gu; g.ld_aux = 2 * F;
@@ -912,14 +954,20 @@ int fwd_bwd(dtx_trainer* t, bool backward) {
       CK(rmsnorm_dw(t->dh, y.x_mid, y.rstd2, M, d, t->ndw_scratch, gl_w + t->off_n2, accumulate, s), 2);
     }
     CK(rmsnorm_bwd(t->dh, y.x_mid, y.norm2, y.rstd2, cur, other, M, d, s), 1);  // other = d x_mid
+    const bf16* d_o = other;  // gradient of the o-projection output
+    if (y.pn) {  // through post_self_attn_layernorm: d o_pre into dh (free until the dh1 GEMM below)
+      if (t->full) CK(rmsnorm_dw(other, y.o_pre, y.rstd_pn1, M, d, t->ndw_scratch, gl_w + t->off_pn, accumulate, s), 2);
+      CK(rmsnorm_bwd(other, y.o_pre, y.pn, y.rstd_pn1, nullptr, t->dh, M, d, s), 1);
+      d_o = t->dh;
+    }
     {  // dattn = dx_mid * Wo
       BASEW(W_O, wo);
       GemmArgs g;
-      g.A = other; g.lda = d; g.B = wo; g.ldb = dq; g.b_mn_major = 1; g.C = t->dattn; g.ldc = dq;
+      g.A = d_o; g.lda = d; g.B = wo; g.ldb = dq; g.b_mn_major = 1; g.C = t->dattn; g.ldc = dq;
       g.M = M; g.N = dq; g.K = d; g.epilogue = EPI_BF16;
       CK(gemm_bf16(g, s), 1);
     }
-    if (t->full) CK(dw_gemm(other, d, y.attn, dq, gl_w + t->off_wo), 1);  // dWo = d x_mid^T * attn
+    if (t->full) CK(dw_gemm(d_o, d, y.attn, dq, gl_w + t->off_wo), 1);  // dWo = d x_mid^T * attn
     {
       AttnArgs a;
       a.qkv = y.qkv; a.out = y.attn; a.lse = y.lse; a.B = B; a.S = S; a.H = H; a.Hkv = Hkv; a.scale = att_scale;
@@ -931,8 +979,10 @@ int fwd_bwd(dtx_trainer* t, bool backward) {
       // (32 uncoalesced 8-byte reads per thread) cost +270 us/layer, the standalone HBM-bound kernel 92 us.
       const bool rope_in_attn = fused && attn_bwd_can_rope();
       a.rope_cs = rope_in_attn ? t->rope_cs_t : nullptr;
+      a.rope_glm = t->rope_glm ? 1 : 0;
       CK(attn_bwd(a, s), attn_bwd_launches());
-      if (!rope_in_attn) CK(rope_qk_inplace_table(t->dqkv, t->rope_cs, B, S, H + Hkv, W, D, 1, s), 1);
+      if (!rope_in_attn && t->rope_glm) CK(rope_glm_qk_inplace(t->dqkv, t->rope_cs, B, S, H + Hkv, W, 1, s), 1);
+      else if (!rope_in_attn) CK(rope_qk_inplace_table(t->dqkv, t->rope_cs, B, S, H + Hkv, W, D, 1, s), 1);
     }
     if (y.qkn) {  // through the q/k norm (Qwen3), in place on the q|k columns of dqkv; full-parameter SFT: d q_norm | d k_norm
       // the dw partials: at most as many 256-float blocks as ndw_scratch (64 * d floats) holds
@@ -1383,7 +1433,7 @@ int check_cfg(const dtx_model_cfg* mc, const dtx_train_cfg* tc) {
 }
 
 // checks of the model-family extensions (host only; the message goes to g_error)
-int check_ext(const dtx_model_ext* ext) {
+int check_ext(const dtx_model_cfg* mc, const dtx_model_ext* ext) {
   if (!ext) return DTX_OK;
   auto bad = [&](const char* m) {
     g_error = m;
@@ -1391,6 +1441,11 @@ int check_ext(const dtx_model_ext* ext) {
   };
   if (ext->qkv_bias != 0 && ext->qkv_bias != 1) return bad("qkv_bias must be 0 or 1");
   if (ext->qk_norm != 0 && ext->qk_norm != 1) return bad("qk_norm must be 0 or 1");
+  if (ext->rope_glm != 0 && ext->rope_glm != 1) return bad("rope_glm must be 0 or 1");
+  if (ext->rope_glm && ext->qk_norm) return bad("rope_glm cannot be combined with qk_norm");
+  if (ext->rope_glm && mc->sliding_window > 0) return bad("rope_glm cannot be combined with a sliding window");
+  if (ext->post_norms != 0 && ext->post_norms != 1) return bad("post_norms must be 0 or 1");
+  if (ext->rope_glm && ext->rope_type != DTX_ROPE_DEFAULT) return bad("rope_glm needs rope_type DTX_ROPE_DEFAULT (no scaled GLM rotary is implemented)");
   if (ext->rope_type < DTX_ROPE_DEFAULT || ext->rope_type > DTX_ROPE_LLAMA3)
     return bad("rope_type must be DTX_ROPE_DEFAULT, DTX_ROPE_LINEAR or DTX_ROPE_LLAMA3 (yarn, dynamic, longrope are not implemented)");
   if (ext->rope_type != DTX_ROPE_DEFAULT && !(ext->rope_factor > 0.0f)) return bad("rope_factor must be > 0");
@@ -1408,6 +1463,8 @@ void setup_dims(dtx_trainer* t, const dtx_model_cfg* mc, const dtx_model_ext* ex
   if (ext) t->ext = *ext;
   t->qkv_bias = t->ext.qkv_bias != 0;
   t->qk_norm = t->ext.qk_norm != 0;
+  t->rope_glm = t->ext.rope_glm != 0;
+  t->post_norms = t->ext.post_norms != 0;
   t->tc = *tc;
   t->world = world;
   t->M = tc->micro_batch * tc->seq_len;
@@ -1508,7 +1565,7 @@ int32_t dtx_rope_inv_freq(const dtx_model_cfg* mc, const dtx_model_ext* ext, flo
     g_error = "rope_inv_freq: head_dim must be a positive even number";
     return DTX_ERR_INVALID;
   }
-  int rc = check_ext(ext);
+  int rc = check_ext(mc, ext);
   if (rc) return rc;
   dtx_model_ext e{};
   if (ext) e = *ext;
@@ -1524,7 +1581,7 @@ int32_t dtx_trainer_create_ext(const dtx_model_cfg* mc, const dtx_model_ext* ext
   }
   *out = nullptr;
   int rc = check_cfg(mc, tc);
-  if (rc == DTX_OK) rc = check_ext(ext);
+  if (rc == DTX_OK) rc = check_ext(mc, ext);
   if (rc) return rc;
   if (world < 1 || rank < 0 || rank >= world) {
     g_error = "bad rank/world";
@@ -1741,9 +1798,31 @@ int32_t dtx_load_tensor(dtx_trainer* t, const char* name, const void* host, int3
     if (rc == DTX_OK) t->qkn_loaded[2 * static_cast<size_t>(layer) + i] = 1;
     return rc;
   }
+  for (int i = 0; i < 2; ++i) {  // Glm4 post-sublayer norms [d]: one [2 * d] vector per layer (bf16 also under NF4)
+    if (!strstr(rest, i ? "post_mlp_layernorm.weight" : "post_self_attn_layernorm.weight")) continue;
+    if (!t->post_norms) return t->fail(DTX_ERR_INVALID, "%s: this trainer was created without post-sublayer norms (dtx_model_ext.post_norms)", name);
+    if (nd != 1 || rows != d) return t->fail(DTX_ERR_INVALID, "%s: expected [%lld]", name, (long long)d);
+    int rc = upload(y.pn + i * d, d);
+    if (rc == DTX_OK) t->pn_loaded[2 * static_cast<size_t>(layer) + i] = 1;
+    return rc;
+  }
   if (t->quant4 && !strstr(rest, "layernorm"))
     return t->fail(DTX_ERR_STATE, "%s: the base weights are already NF4-packed; load tensors before dtx_quantize_base", name);
   // gate/up rows go to the GU-interleaved layout: 128 gate rows, then the 128 up rows of the same features, ...
+  if (strstr(rest, "mlp.gate_up_proj.weight")) {  // GLM's fused [gate F | up F] rows (modeling_glm GlmMLP: chunk(2))
+    if (!expect(2 * F, d)) return t->fail(DTX_ERR_INVALID, "%s: expected [%lld,%lld]", name, (long long)(2 * F), (long long)d);
+    std::vector<bf16> tmp;
+    to_bf16_host(host, dtype, static_cast<size_t>(2 * F) * d, tmp);
+    for (int which = 0; which < 2; ++which)
+      for (int64_t b = 0; b < F / 128; ++b) {
+        cudaError_t e = cudaMemcpyAsync(y.wgu + (b * 256 + which * 128) * d, tmp.data() + (which * F + b * 128) * d,
+                                        128 * d * sizeof(bf16), cudaMemcpyHostToDevice, t->stream);
+        if (e != cudaSuccess) return t->fail(DTX_ERR_CUDA, "upload %s: %s", name, cudaGetErrorString(e));
+      }
+    CKM(cudaStreamSynchronize(t->stream));  // `tmp` dies at the end of this scope
+    lmap[4] = lmap[5] = 1;
+    return DTX_OK;
+  }
   for (int which = 0; which < 2; ++which) {
     if (!strstr(rest, which ? "mlp.up_proj.weight" : "mlp.gate_proj.weight")) continue;
     if (!expect(F, d)) return t->fail(DTX_ERR_INVALID, "%s: expected [%lld,%lld]", name, (long long)F, (long long)d);
@@ -1796,12 +1875,14 @@ int32_t dtx_init_random_weights(dtx_trainer* t, uint64_t seed) {
     CK(fill_const_bf16(y.norm2, d, 1.0f, s), 1);
     if (y.bias) CK(fill_const_bf16(y.bias, t->W, 0.0f, s), 1);  // HF _init_weights zeroes Linear biases
     if (y.qkn) CK(fill_const_bf16(y.qkn, 2 * t->mc.head_dim, 1.0f, s), 1);  // ... and sets RMSNorm weights to 1
+    if (y.pn) CK(fill_const_bf16(y.pn, 2 * d, 1.0f, s), 1);
   }
   cudaError_t e = cudaStreamSynchronize(s);
   if (e != cudaSuccess) return t->fail(DTX_ERR_CUDA, "init_random_weights: %s", cudaGetErrorString(e));
   std::fill(t->loaded.begin(), t->loaded.end(), 1);
   std::fill(t->bias_loaded.begin(), t->bias_loaded.end(), 1);
   std::fill(t->qkn_loaded.begin(), t->qkn_loaded.end(), 1);
+  std::fill(t->pn_loaded.begin(), t->pn_loaded.end(), 1);
   return DTX_OK;
 }
 
@@ -2146,6 +2227,15 @@ int32_t dtx_export_weight(dtx_trainer* t, const char* name, void* host_out, int6
   }
   if (layer < 0 || layer >= L) return t->fail(DTX_ERR_INVALID, "%s: layer out of range", name);
   const bf16* blk = flat + layer * t->layer_elems;
+  if (strstr(rest, "mlp.gate_up_proj.weight")) {  // the fused HF tensor: all gate rows, then all up rows
+    if (nbytes < 2 * F * d * 2) return t->fail(DTX_ERR_INVALID, "%s: output buffer too small", name);
+    for (int which = 0; which < 2; ++which)
+      for (int64_t b = 0; b < F / 128; ++b)
+        CKM(cudaMemcpyAsync(static_cast<bf16*>(host_out) + (which * F + b * 128) * d, blk + t->off_wgu + (b * 256 + which * 128) * d,
+                            128 * d * 2, cudaMemcpyDeviceToHost, t->stream));
+    CKM(cudaStreamSynchronize(t->stream));
+    return DTX_OK;
+  }
   for (int which = 0; which < 2; ++which) {
     if (!strstr(rest, which ? "mlp.up_proj.weight" : "mlp.gate_proj.weight")) continue;
     if (nbytes < F * d * 2) return t->fail(DTX_ERR_INVALID, "%s: output buffer too small", name);
@@ -2177,6 +2267,10 @@ int32_t dtx_export_weight(dtx_trainer* t, const char* name, void* host_out, int6
     if (strstr(rest, "self_attn.q_norm.weight")) return copy(blk + t->off_qkn, D);
     if (strstr(rest, "self_attn.k_norm.weight")) return copy(blk + t->off_qkn + D, D);
   }
+  if (t->post_norms) {
+    if (strstr(rest, "post_self_attn_layernorm.weight")) return copy(blk + t->off_pn, d);
+    if (strstr(rest, "post_mlp_layernorm.weight")) return copy(blk + t->off_pn + d, d);
+  }
   return t->fail(DTX_ERR_INVALID, "unknown tensor name %s", name);
 }
 
@@ -2198,7 +2292,7 @@ int32_t dtx_plan_device_bytes_ext(const dtx_model_cfg* mc, const dtx_model_ext* 
     return DTX_ERR_INVALID;
   }
   int rc = check_cfg(mc, tc);
-  if (rc == DTX_OK) rc = check_ext(ext);
+  if (rc == DTX_OK) rc = check_ext(mc, ext);
   if (rc) return rc;
   *bytes_out = planned_bytes(mc, ext, tc, world, 132, layout);  // split-K buffers sized for the 132 SMs of an H100 SXM
   return DTX_OK;

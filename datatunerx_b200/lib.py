@@ -43,7 +43,8 @@ class ModelCfg(C.Structure):
 class ModelExt(C.Structure):
     _fields_ = [("qkv_bias", C.c_int32), ("rope_type", C.c_int32), ("rope_factor", C.c_float),
                 ("rope_low_freq_factor", C.c_float), ("rope_high_freq_factor", C.c_float), ("rope_original_max_pos", C.c_int32),
-                ("qk_norm", C.c_int32)]
+                ("qk_norm", C.c_int32), ("rope_glm", C.c_int32),
+                ("post_norms", C.c_int32)]
 
 
 class TrainCfg(C.Structure):
@@ -59,7 +60,7 @@ class TrainCfg(C.Structure):
 ABI_SYMBOLS = [
     "dtx_abi_version", "dtx_last_global_error", "dtx_last_error", "dtx_trainer_create", "dtx_trainer_create_ext",
     "dtx_rope_inv_freq", "dtx_plan_device_bytes_ext", "dtx_gemm_bias", "dtx_bias_grad", "dtx_gemm_qk_norm", "dtx_qk_norm_fwd",
-    "dtx_qk_norm_bwd", "dtx_trainer_destroy",
+    "dtx_qk_norm_bwd", "dtx_gemm_rope_glm", "dtx_rope_glm_qk", "dtx_attn_bwd_rope", "dtx_post_norm_add", "dtx_trainer_destroy",
     "dtx_get_nccl_unique_id", "dtx_load_tensor", "dtx_init_random_weights", "dtx_init_lora", "dtx_quantize_base", "dtx_step",
     "dtx_step_device", "dtx_eval_loss", "dtx_allreduce_host", "dtx_export_adapter", "dtx_export_adapter_grad", "dtx_export_weight", "dtx_num_trainable", "dtx_launch_count",
     "dtx_recompute", "dtx_device_bytes", "dtx_plan_device_bytes",
@@ -99,6 +100,10 @@ def load() -> C.CDLL:
                                      i32, vp, vp, C.c_float, vp]
     lib.dtx_qk_norm_fwd.argtypes = [vp, i64, i32, i32, i32, vp, vp, C.c_float, vp, i64, vp]
     lib.dtx_qk_norm_bwd.argtypes = [vp, i64, vp, i64, i32, i32, i32, vp, vp, C.c_float, vp, vp, i32, i32, vp]
+    lib.dtx_gemm_rope_glm.argtypes = [vp, i64, vp, i64, i32, vp, i64, vp, i64, i32, vp, i64, vp, i32, i32, vp, i32, i32, i32, vp, vp]
+    lib.dtx_rope_glm_qk.argtypes = [vp, vp, i32, i32, i32, i32, i32, vp]
+    lib.dtx_attn_bwd_rope.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, f32, vp, i32, vp, i32, i32, vp]
+    lib.dtx_post_norm_add.argtypes = [vp, vp, vp, vp, vp, i32, i32, C.c_float, vp]
     lib.dtx_trainer_destroy.argtypes = [vp]
     lib.dtx_trainer_destroy.restype = None
     lib.dtx_get_nccl_unique_id.argtypes = [vp]
@@ -207,10 +212,10 @@ def plan_device_bytes(model: "ModelConfig", train: "TrainConfig", world: int = 1
 
 
 def rope_inv_freq(model: "ModelConfig") -> np.ndarray:
-    """The fp32 inverse frequencies the trainer builds its rotary table from (head_dim / 2 values; host arithmetic inside the
-    library, no GPU needed)."""
+    """The fp32 inverse frequencies the trainer builds its rotary table from (head_dim / 2 values, head_dim / 4 with GLM's partial
+    rotary; host arithmetic inside the library, no GPU needed)."""
     mc, ext = model.to_c(), model.ext_to_c()
-    out = np.zeros(model.head_dim // 2, np.float32)
+    out = np.zeros(model.head_dim // (4 if model.rope_glm else 2), np.float32)
     check(load().dtx_rope_inv_freq(C.byref(mc), C.byref(ext), out.ctypes.data_as(C.c_void_p)))
     return out
 
@@ -235,6 +240,10 @@ class ModelConfig:
     sliding_window: int = 0            # Mistral config.json `sliding_window`; 0 = none
     qkv_bias: bool = False             # q_proj / k_proj / v_proj carry a bias (Qwen2)
     qk_norm: bool = False              # RMSNorm over every q / k head before the rotary (Qwen3 q_norm / k_norm)
+    # GLM (GlmForCausalLM): partial interleaved rotary over the first half of every q / k head; its checkpoints also store
+    # gate_proj | up_proj as one mlp.gate_up_proj tensor, the name weight_names / export_weights use for it
+    rope_glm: bool = False
+    post_norms: bool = False           # Glm4 post_self_attn_layernorm / post_mlp_layernorm after the two sublayers
     # HF config.json `rope_scaling` / `rope_parameters`: {"rope_type" (or the older "type"): "linear" | "llama3", "factor", ...};
     # None = the plain theta table
     rope_scaling: Optional[dict] = None
@@ -252,11 +261,11 @@ class ModelConfig:
         kind = rs.get("rope_type", rs.get("type", "default"))
         if kind not in ROPE_TYPES:
             raise DtxError(-1, f"rope_type {kind!r}: only {', '.join(ROPE_TYPES)} are implemented natively")
-        qkn = int(bool(self.qk_norm))
+        qkn, glm, pn = int(bool(self.qk_norm)), int(bool(self.rope_glm)), int(bool(self.post_norms))
         if kind == "default":
-            return ModelExt(int(bool(self.qkv_bias)), 0, 0.0, 0.0, 0.0, 0, qkn)
+            return ModelExt(int(bool(self.qkv_bias)), 0, 0.0, 0.0, 0.0, 0, qkn, glm, pn)
         return ModelExt(int(bool(self.qkv_bias)), ROPE_TYPES[kind], float(rs["factor"]), float(rs.get("low_freq_factor", 0.0)),
-                        float(rs.get("high_freq_factor", 0.0)), int(rs.get("original_max_position_embeddings", 0)), qkn)
+                        float(rs.get("high_freq_factor", 0.0)), int(rs.get("original_max_position_embeddings", 0)), qkn, glm, pn)
 
 
 @dataclass
@@ -437,18 +446,24 @@ class Trainer:
             yield p + "self_attn.k_proj.weight", (dkv, d)
             yield p + "self_attn.v_proj.weight", (dkv, d)
             if m.qkv_bias:
-                yield p + "self_attn.q_proj.bias", (d,)
+                yield p + "self_attn.q_proj.bias", (dq,)
                 yield p + "self_attn.k_proj.bias", (dkv,)
                 yield p + "self_attn.v_proj.bias", (dkv,)
             if m.qk_norm:
                 yield p + "self_attn.q_norm.weight", (m.head_dim,)
                 yield p + "self_attn.k_norm.weight", (m.head_dim,)
             yield p + "self_attn.o_proj.weight", (d, dq)
-            yield p + "mlp.gate_proj.weight", (F, d)
-            yield p + "mlp.up_proj.weight", (F, d)
+            if m.rope_glm:
+                yield p + "mlp.gate_up_proj.weight", (2 * F, d)
+            else:
+                yield p + "mlp.gate_proj.weight", (F, d)
+                yield p + "mlp.up_proj.weight", (F, d)
             yield p + "mlp.down_proj.weight", (d, F)
             yield p + "input_layernorm.weight", (d,)
             yield p + "post_attention_layernorm.weight", (d,)
+            if m.post_norms:
+                yield p + "post_self_attn_layernorm.weight", (d,)
+                yield p + "post_mlp_layernorm.weight", (d,)
         yield "model.norm.weight", (d,)
         yield "lm_head.weight", (V, d)
 

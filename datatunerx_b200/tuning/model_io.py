@@ -1,7 +1,9 @@
 """Model / adapter file IO of the worker, numpy only (no torch, no safetensors package needed at run time).
 
   * load_model_config  : HF config.json -> ModelConfig  (AutoConfig.from_pretrained, cmd/tuning/train.py:221): Llama-2,
-                         Llama-3.x (linear / llama3 rope scaling), Mistral, Qwen2 / Qwen2.5 (q/k/v biases), Qwen3 (q/k norm)
+                         Llama-3.x (linear / llama3 rope scaling), Mistral, Qwen2 / Qwen2.5 (q/k/v biases), Qwen3 (q/k norm),
+                         GLM-4 (GlmForCausalLM / Glm4ForCausalLM: partial interleaved rotary, q/k/v biases,
+                         fused gate_up_proj, Glm4's post-sublayer norms)
   * iter_safetensors   : stream tensors of *.safetensors shards (AutoModelForCausalLM.from_pretrained, train.py:236-242);
                          iter_torch_bin does the same for pytorch_model*.bin shards
   * save_peft_adapter  : adapter_config.json + adapter_model.safetensors (+ adapter_model.bin when torch is importable)
@@ -29,14 +31,20 @@ _ROPE_TYPES = ("default", "linear", "llama3")
 
 def load_model_config(model_dir: str, full_finetune: bool = False) -> ModelConfig:
     """HF config.json -> ModelConfig for the decoders the library trains: Llama-2 / Llama-3.x (`rope_scaling` of type linear or
-    llama3), Mistral, Qwen2 / Qwen2.5 (q/k/v biases) and Qwen3 (q/k RMSNorm, attention width n_heads * head_dim != hidden).
+    llama3), Mistral, Qwen2 / Qwen2.5 (q/k/v biases), Qwen3 (q/k RMSNorm, attention width n_heads * head_dim != hidden) and
+    GLM-4 (glm-4-9b-hf, GLM-4-0414, GLM-Z1: GLM's partial interleaved rotary, q/k/v biases from `attention_bias`, and for
+    Glm4ForCausalLM the post-sublayer norms).
     Anything that would train a different model than HF's raises ValueError."""
     cfg = json.load(open(os.path.join(model_dir, "config.json")))
     arch = (cfg.get("architectures") or ["LlamaForCausalLM"])[0]
     qwen2, qwen3 = arch == "Qwen2ForCausalLM", arch == "Qwen3ForCausalLM"
-    if "Llama" not in arch and "Mistral" not in arch and not qwen2 and not qwen3:
-        raise ValueError(f"{arch}: only Llama-family, Qwen2 and Qwen3 decoders are implemented natively")
-    if cfg.get("attention_bias") or cfg.get("mlp_bias"):
+    glm4 = arch == "Glm4ForCausalLM"
+    glm = arch == "GlmForCausalLM" or glm4
+    if "Llama" not in arch and "Mistral" not in arch and not qwen2 and not qwen3 and not glm:
+        raise ValueError(f"{arch}: only Llama-family, Qwen2, Qwen3 and GLM decoders are implemented natively")
+    if glm:
+        _check_glm(cfg, full_finetune)
+    elif cfg.get("attention_bias") or cfg.get("mlp_bias"):
         raise ValueError(f"{arch}: attention_bias / mlp_bias are not implemented natively")
     # transformers 5 names the dict `rope_parameters` (it then also carries rope_theta); older configs `rope_scaling`
     rs = cfg.get("rope_scaling") or cfg.get("rope_parameters") or None
@@ -47,6 +55,8 @@ def load_model_config(model_dir: str, full_finetune: bool = False) -> ModelConfi
             raise ValueError(f"rope_scaling type {kind!r} is not implemented natively (supported: {', '.join(_ROPE_TYPES)})")
         rs = None if kind == "default" else dict(rs)
     window = int(cfg.get("sliding_window") or 0)
+    if glm and rs is not None:
+        raise ValueError(f"{arch}: rope scaling {rs.get('rope_type', rs.get('type'))!r} of GLM's partial rotary is not implemented natively")
     if qwen2 or qwen3:
         # Qwen2.5 / Qwen3 ship sliding_window with use_sliding_window = false: HF then attends over the whole causal window
         name = "Qwen2" if qwen2 else "Qwen3"
@@ -60,8 +70,23 @@ def load_model_config(model_dir: str, full_finetune: bool = False) -> ModelConfi
     return ModelConfig(vocab=cfg["vocab_size"], hidden=cfg["hidden_size"], n_layers=cfg["num_hidden_layers"], n_heads=heads,
                        n_kv_heads=cfg.get("num_key_value_heads", heads), head_dim=cfg.get("head_dim") or cfg["hidden_size"] // heads,
                        ffn=cfg["intermediate_size"], rms_eps=cfg.get("rms_norm_eps", 1e-5), rope_theta=rope_theta,
-                       max_seq=cfg.get("max_position_embeddings", 4096), sliding_window=window, qkv_bias=qwen2, qk_norm=qwen3,
+                       max_seq=cfg.get("max_position_embeddings", 4096), sliding_window=window,
+                       qkv_bias=qwen2 or (glm and bool(cfg.get("attention_bias", True))), qk_norm=qwen3, rope_glm=glm, post_norms=glm4,
                        rope_scaling=rs)
+
+
+def _check_glm(cfg: dict, full_finetune: bool) -> None:
+    """What GlmForCausalLM may carry and still be the model the library trains (transformers modeling_glm)."""
+    prf = cfg.get("partial_rotary_factor", (cfg.get("rope_parameters") or {}).get("partial_rotary_factor", 0.5))
+    if prf != 0.5:
+        raise ValueError(f"GLM partial_rotary_factor {prf}: only 0.5 (half of every head rotated) is implemented natively")
+    if cfg.get("hidden_act", "silu") != "silu":
+        raise ValueError(f"GLM hidden_act {cfg.get('hidden_act')!r}: only silu is implemented natively")
+    if cfg.get("mlp_bias"):
+        raise ValueError("GLM mlp_bias is not implemented natively")
+    if full_finetune and cfg.get("tie_word_embeddings"):
+        raise ValueError("full-parameter SFT of a GLM checkpoint with tie_word_embeddings would train the embedding and lm_head as "
+                         "two tensors, unlike HF; use LoRA")
 
 
 def check_attention_window(model_dir: str, seq_len: int) -> None:

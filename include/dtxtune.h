@@ -88,9 +88,10 @@ typedef struct {
 } dtx_train_cfg;
 
 /* Model-family extensions of dtx_model_cfg (Llama-3.1 / 3.2 scaled rotary tables, Qwen2 q/k/v projection biases, Qwen3 q/k
- * RMSNorm).  A NULL or all-zero dtx_model_ext is the plain Llama-2 / Mistral model: no bias, no q/k norm, rotary inverse
- * frequencies theta^(-2i/D).  qk_norm was appended after the struct's first release: C callers must be rebuilt against this
- * header (a caller compiled against the shorter struct passes a struct the library reads one field past). */
+ * RMSNorm, GLM's partial interleaved rotary, Glm4's post-sublayer norms).  A NULL or all-zero dtx_model_ext is the plain Llama-2 / Mistral model: no bias,
+ * no q/k norm, rotary inverse frequencies theta^(-2i/D) over the whole head.  qk_norm, rope_glm and post_norms were appended after the
+ * struct's first release: C callers must be rebuilt against this header (a caller compiled against a shorter struct passes a
+ * struct the library reads past). */
 #define DTX_ROPE_DEFAULT 0   /* inv_freq = theta^(-2i/D) */
 #define DTX_ROPE_LINEAR  1   /* inv_freq / factor (HF rope_type "linear") */
 #define DTX_ROPE_LLAMA3  2   /* HF _compute_llama3_parameters (Llama-3.1 / 3.2): high frequencies kept, low ones / factor,
@@ -101,6 +102,13 @@ typedef struct {
   float rope_factor, rope_low_freq_factor, rope_high_freq_factor;  /* factor: linear and llama3; the two others: llama3 */
   int32_t rope_original_max_pos;    /* llama3: original_max_position_embeddings */
   int32_t qk_norm;                  /* 1: RMSNorm over every q and k head before the rotary (Qwen3 q_norm / k_norm, eps = rms_eps) */
+  int32_t rope_glm;                 /* 1: GLM's rotary (GlmForCausalLM, partial_rotary_factor 0.5): only the first head_dim / 2
+                                       dims of every q / k head turn, in adjacent pairs (2i, 2i + 1) with inv_freq[i] =
+                                       theta^(-2i / (head_dim / 2)); the other half passes through.  Not with qk_norm, and
+                                       rope_type must be DTX_ROPE_DEFAULT */
+  int32_t post_norms;               /* 1: Glm4's post-sublayer norms (Glm4ForCausalLM): post_self_attn_layernorm RMS-normalises
+                                       the o_proj output and post_mlp_layernorm the down_proj output before their residual adds
+                                       (eps = rms_eps) */
 } dtx_model_ext;
 
 typedef struct dtx_trainer dtx_trainer;
@@ -116,8 +124,12 @@ DTX_API const char* dtx_last_error(const dtx_trainer* t);
 DTX_API int32_t dtx_trainer_create(const dtx_model_cfg* model, const dtx_train_cfg* train, int32_t device, int32_t rank,
                            int32_t world, const void* nccl_unique_id, dtx_trainer** out);
 /* The same for a model with family extensions (ext may be NULL: dtx_trainer_create).  An unknown rope_type, a factor <= 0, or
- * for llama3 low_freq_factor >= high_freq_factor or original_max_pos <= 0, or qkv_bias / qk_norm other than 0 / 1 return
- * DTX_ERR_INVALID before any device work.
+ * for llama3 low_freq_factor >= high_freq_factor or original_max_pos <= 0, or qkv_bias / qk_norm / rope_glm other than 0 / 1,
+ * or rope_glm with qk_norm, with a rope_type other than DTX_ROPE_DEFAULT or with a sliding window, or post_norms other than
+ * 0 / 1 return DTX_ERR_INVALID before any device work.  With post_norms, "model.layers.N.post_self_attn_layernorm.weight" and
+ * "model.layers.N.post_mlp_layernorm.weight" [hidden] follow the rules of the q/k norm weights below.
+ * "model.layers.N.mlp.gate_up_proj.weight" [2 * ffn, hidden] (GLM: gate rows, then up rows) loads in place of gate_proj and
+ * up_proj for any model; dtx_export_weight returns it under that name too.
  * With qkv_bias, "model.layers.N.self_attn.{q,k,v}_proj.bias" must be loaded before a step; full-parameter SFT trains them
  * without weight decay (HF get_decay_parameter_names), LoRA keeps them frozen (peft bias="none").  With qk_norm, the same holds
  * for "model.layers.N.self_attn.{q,k}_norm.weight" [head_dim].
@@ -125,7 +137,8 @@ DTX_API int32_t dtx_trainer_create(const dtx_model_cfg* model, const dtx_train_c
  * o_proj [hidden, n_heads * head_dim]. */
 DTX_API int32_t dtx_trainer_create_ext(const dtx_model_cfg* model, const dtx_model_ext* ext, const dtx_train_cfg* train,
                                        int32_t device, int32_t rank, int32_t world, const void* nccl_unique_id, dtx_trainer** out);
-/* host arithmetic, no device: the fp32 inverse frequencies the rotary table is built from (head_dim / 2 values) */
+/* host arithmetic, no device: the fp32 inverse frequencies the rotary table is built from (head_dim / 2 values; with rope_glm
+ * head_dim / 4, bitwise transformers' GlmRotaryEmbedding.inv_freq) */
 DTX_API int32_t dtx_rope_inv_freq(const dtx_model_cfg* model, const dtx_model_ext* ext, float* out);
 DTX_API void dtx_trainer_destroy(dtx_trainer* t);
 DTX_API int32_t dtx_get_nccl_unique_id(void* out128);
@@ -286,6 +299,22 @@ DTX_API int32_t dtx_qk_norm_fwd(void* qkv, int64_t ld, int32_t M, int32_t q_cols
 DTX_API int32_t dtx_qk_norm_bwd(void* dy, int64_t ld, const void* x, int64_t ldx, int32_t M, int32_t q_cols, int32_t n_cols,
                                 const void* wq, const void* wk, float eps, void* dw, void* scratch, int32_t nblk, int32_t accumulate,
                                 void* stream);
+/* dtx_gemm_bias's arguments for epilogue 3 (EPI_ROPE), the bias optional (NULL: none), with GLM's partial interleaved rotary:
+ * columns 2i, 2i + 1 (i < 32) of every rotated 128-column head (columns < rope_cols) turn by rope_cs[pos][i] (table [rope_S][32]
+ * float2), columns 64..127 of the head and every column >= rope_cols are the plain (+ bias) projection.  rope_cols and N:
+ * multiples of 256. */
+DTX_API int32_t dtx_gemm_rope_glm(const void* A, int64_t lda, const void* B, int64_t ldb, int32_t b_mn_major, const void* A2,
+                                  int64_t lda2, const void* B2, int64_t ldb2, int32_t K2, void* C, int64_t ldc, const void* rope_cs,
+                                  int32_t rope_S, int32_t rope_cols, const void* rope_pos, int32_t M, int32_t N, int32_t K,
+                                  const void* bias, void* stream);
+/* The same rotary on its own, in place on the H q heads and Hkv k heads of packed qkv [B*S, (H + 2*Hkv)*128] (the unfused path);
+ * cs_table [S][32]; inverse = 1 applies the transposed rotation (backward). */
+DTX_API int32_t dtx_rope_glm_qk(void* qkv, const void* cs_table, int32_t B, int32_t S, int32_t H, int32_t Hkv, int32_t inverse,
+                                void* stream);
+/* Glm4's post-sublayer norm and residual add in one pass over bf16 [M, d] rows: out = res + w * (y * rsqrt(mean(y^2) + eps))
+ * in fp32; rstd (fp32 [M]) is saved for dtx_rmsnorm_bwd(dy, y, w, rstd, dres = NULL).  out = NULL computes rstd only. */
+DTX_API int32_t dtx_post_norm_add(const void* y, const void* w, const void* res, void* out, void* rstd, int32_t M, int32_t d,
+                                  float eps, void* stream);
 DTX_API int32_t dtx_embedding_fwd(const void* ids, const void* table, void* out, int32_t M, int32_t d, int32_t vocab, void* stream);
 DTX_API int32_t dtx_rmsnorm_fwd(const void* x, const void* w, void* y, void* rstd, int32_t M, int32_t d, float eps, void* stream);
 DTX_API int32_t dtx_rmsnorm_bwd(const void* dy, const void* x, const void* w, const void* rstd, const void* dres, void* dx,
@@ -322,6 +351,11 @@ DTX_API int32_t dtx_attn_fwd(const void* qkv, void* out, void* lse2, int32_t B, 
 DTX_API int32_t dtx_attn_bwd(const void* qkv, const void* out, const void* dout, const void* lse2, void* delta_scratch,
                      void* dqkv, int32_t B, int32_t S, int32_t H, int32_t Hkv, float scale, const void* seq_lens,
                      int32_t window, const void* rope_cs_t, int32_t rope_stride, void* stream);
+/* dtx_attn_bwd with a rotary mode for rope_cs_t: rope_glm = 0 is dtx_attn_bwd, 1 applies GLM's inverse rotary (partial,
+ * interleaved) from a transposed [32][rope_stride] table; rope_glm = 1 needs window 0. */
+DTX_API int32_t dtx_attn_bwd_rope(const void* qkv, const void* out, const void* dout, const void* lse2, void* delta_scratch,
+                                  void* dqkv, int32_t B, int32_t S, int32_t H, int32_t Hkv, float scale, const void* seq_lens,
+                                  int32_t window, const void* rope_cs_t, int32_t rope_stride, int32_t rope_glm, void* stream);
 
 #ifdef __cplusplus
 }

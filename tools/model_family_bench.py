@@ -9,6 +9,10 @@
   * The Qwen2.5-7B q|k|v GEMM (M 8192 x N 4608 x K 3584, fused RoPE epilogue) with and without the bias, and the Qwen3-8B one
     (M 8192 x N 6144 x K 4096) with and without the QK-norm epilogue, each pair alternated in one process, timed with CUDA
     events; qk_norm_bwd at the Qwen3-8B shape (time and GB/s of the bytes it must move).
+  * GLM-4-9B-0414 shape (Glm4ForCausalLM: GLM's partial interleaved rotary, q/k/v biases, post-sublayer norms, GQA 32 / 2,
+    FFN 13 696, vocab 151 552; q|k|v width 4608), the same workload.  Its q|k|v GEMM (M 8192 x N 4608 x K 4096) with the GLM
+    epilogue against the half-split EPI_ROPE epilogue, both with the bias, alternated; post_norm_add at M 8192 x d 4096 (time and
+    GB/s); attn_dkv_kernel (torch.profiler) at B 4 x S 2048 with GLM's 32 / 2 heads against Llama-3.1-8B's 32 / 8.
 
 The card's name and power limit are read in the same run and printed with the numbers.  Prints one JSON document; --out also
 writes it to a file.
@@ -42,6 +46,8 @@ CONFIGS = {
                               rms_eps=1e-6, max_seq=40960, qk_norm=True),
     "qwen3-4b": L.ModelConfig(vocab=151936, hidden=2560, n_layers=36, n_heads=32, n_kv_heads=8, ffn=9728, rope_theta=1000000.0,
                               rms_eps=1e-6, max_seq=40960, qk_norm=True),
+    "glm-4-9b-0414": L.ModelConfig(vocab=151552, hidden=4096, n_layers=40, n_heads=32, n_kv_heads=2, ffn=13696, rope_theta=10000.0,
+                                   max_seq=32768, qkv_bias=True, rope_glm=True, post_norms=True),
 }
 
 
@@ -175,6 +181,68 @@ def qk_norm_cost(iters: int, rounds: int) -> dict:
     return res
 
 
+def glm_cost(iters: int, rounds: int) -> dict:
+    """GLM-4-9B: the q|k|v GEMM with GLM's epilogue against the half-split one (both + bias), post_norm_add, and attn_dkv_kernel
+    at 32 / 2 heads against 32 / 8"""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    M, N, K, d = 8192, 4608, 4096, 4096
+    lib = L.load()
+    g = torch.Generator().manual_seed(0)
+    A = (torch.randn(M, K, generator=g) * 0.5).to(torch.bfloat16).cuda()
+    Bw = (torch.randn(N, K, generator=g) * 0.02).to(torch.bfloat16).cuda()
+    bias = (torch.randn(N, generator=g) * 0.1).to(torch.bfloat16).cuda()
+    Cm = torch.empty(M, N, dtype=torch.bfloat16, device="cuda")
+    cs = torch.empty(S_ROPE, 64, 2, dtype=torch.float32, device="cuda")  # the half-split table; GLM reads its first S x 32 pairs
+    stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+    L.check(lib.dtx_rope_table(C.c_void_p(cs.data_ptr()), S_ROPE, 128, 10000.0, stream))
+    P = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None  # noqa: E731
+    QK = 34 * 128
+
+    def gemm(glm: bool):
+        L.check(lib.dtx_gemm_rope_glm(P(A), K, P(Bw), K, 0, None, 0, None, 0, 0, P(Cm), N, P(cs), S_ROPE, QK, None, M, N, K, P(bias),
+                                      stream) if glm else
+                lib.dtx_gemm_bias(P(A), K, P(Bw), K, 0, None, 0, None, 0, 0, P(Cm), N, None, 0, P(cs), S_ROPE, QK, None, M, N, K,
+                                  L.EPI_ROPE, P(bias), stream))
+
+    times = _alternate(gemm, (False, True), iters, rounds)
+    flop = 2.0 * M * N * K
+    res = {"gemm_shape": [M, N, K]}
+    for glm, key in ((False, "rope_bias"), (True, "rope_glm_bias")):
+        ms = statistics.median(times[glm])
+        res[key] = {"ms_median": ms, "ms_range": [min(times[glm]), max(times[glm])], "tflops": flop / ms / 1e9}
+    y, res_in = A[:, :d].contiguous(), A[:, :d].contiguous()
+    w = (1 + torch.randn(d, generator=g) * 0.1).to(torch.bfloat16).cuda()
+    out, rstd = torch.empty(M, d, dtype=torch.bfloat16, device="cuda"), torch.empty(M, dtype=torch.float32, device="cuda")
+    pn = _alternate(lambda _: L.check(lib.dtx_post_norm_add(P(y), P(w), P(res_in), P(out), P(rstd), M, d, 1e-5, stream)), (0,), iters,
+                    rounds)[0]
+    ms = statistics.median(pn)
+    nbytes = 3 * M * d * 2 + 4 * M
+    res["post_norm_add"] = {"shape": [M, d], "ms_median": ms, "ms_range": [min(pn), max(pn)], "bytes": nbytes, "gb_per_s": nbytes / ms / 1e6}
+    B, S, H = 4, 2048, 32
+    for hkv, key in ((2, "attn_dkv_32_2"), (8, "attn_dkv_32_8")):
+        W = (H + 2 * hkv) * 128
+        qkv = (torch.randn(B * S, W, generator=g) * 0.5).to(torch.bfloat16).cuda()
+        o, do = torch.empty(B * S, H * 128, dtype=torch.bfloat16, device="cuda"), (torch.randn(B * S, H * 128, generator=g) * 0.1).to(torch.bfloat16).cuda()
+        lse, delta = torch.empty(B, H, S, dtype=torch.float32, device="cuda"), torch.empty(B, H, S, dtype=torch.float32, device="cuda")
+        dqkv = torch.empty(B * S, W, dtype=torch.bfloat16, device="cuda")
+        sc = 1.0 / 128 ** 0.5
+        L.check(lib.dtx_attn_fwd(P(qkv), P(o), P(lse), B, S, H, hkv, sc, None, 0, stream))
+        bwd = lambda: L.check(lib.dtx_attn_bwd(P(qkv), P(o), P(do), P(lse), P(delta), P(dqkv), B, S, H, hkv, sc, None, 0, None, 0,  # noqa: E731
+                                               stream))
+        for _ in range(5):
+            bwd()
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(iters):
+                bwd()
+            torch.cuda.synchronize()
+        ev = [e for e in prof.key_averages() if "attn_dkv_kernel" in e.key]
+        res[key] = {"ms_mean": sum(e.device_time_total for e in ev) / max(1, sum(e.count for e in ev)) / 1e3,
+                    "grid_ctas": B * hkv * (S // 128)}
+    return res
+
+
 S_ROPE = 2048
 
 
@@ -194,6 +262,7 @@ def main() -> None:
         print(json.dumps(res["runs"][-1]), flush=True)
     res["qkv_gemm_bias_cost"] = bias_gemm_cost(iters=50, rounds=6)
     res["qkv_gemm_qk_norm_cost"] = qk_norm_cost(iters=50, rounds=6)
+    res["glm_cost"] = glm_cost(iters=50, rounds=6)
     res["card_after"] = card()
     print(json.dumps(res, indent=1))
     if a.out:
