@@ -624,6 +624,12 @@ attn_dkv_kernel(const __grid_constant__ CUtensorMap tmKV128, const __grid_consta
     const int qs = (i0 + qi) * 64;
     if (++qi == nq) qi = 0;
     if (qs + 63 < kw0 || (WIN && qs > kw0 + 63 + window)) {  // no query of the block sees a key of this warpgroup
+      // Wait for the pair's loads all the same: the producer re-arms the slot once all eight warps have released it, so a
+      // warpgroup that released skipped pairs without waiting could also release the slot's next use (warpgroup 1 skips the
+      // first query block of every head of the group) and the producer would re-arm bar_q while those loads are in flight.
+      // A plain spin: the watchdog's trap path here makes ptxas move the dK / dV accumulators to the stack.  It cannot hang on
+      // its own - the producer issues pair ii as soon as every warp has released pair ii - DKV_NS.
+      while (!mbar_try_wait(&bar_q[slot], (ii / DKV_NS) & 1)) {}
       if (lane == 0) mbar_arrive(&bar_free[slot]);
       continue;
     }
