@@ -165,6 +165,36 @@ struct Layer {
   float* absmax[4] = {nullptr, nullptr, nullptr, nullptr};
 };
 enum { W_QKV = 0, W_O = 1, W_GU = 2, W_DOWN = 3 };
+
+// One storage slot of a weight block.  dtx_trainer::lslots lists a decoder layer's slots and dtx_trainer::gslots the globals'
+// (embed | lm_head | final norm); a tensor only some model families have is a row of its own, absent for the others.  Both
+// tables are built once by setup_dims(), and every fact about a block comes from them: full-parameter SFT lays the block out
+// in row order, LoRA allocates the slots one by one in that order, and the memory plan, loading, export, random init and NF4
+// quantisation walk the rows.
+enum { INIT_NORMAL, INIT_ZERO, INIT_ONE };  // dtx_init_random_weights: normal(0.02) with the next seed, 0 (biases), 1 (norms)
+template <class Owner>
+struct Slot {
+  using Ptr = bf16* Owner::*;
+  Ptr mem;            // the pointer this slot fills (Layer::wqkv, ..., dtx_trainer::embed, ...)
+  int64_t n;          // elements
+  int64_t off;        // offset inside the full-SFT block
+  bool nodecay;       // no weight decay (HF get_decay_parameter_names skips biases and norm weights): such rows come last
+  int nf4;            // W_QKV .. W_DOWN: NF4-packed by dtx_quantize_base (index of Layer::q4 / absmax); -1: always bf16
+  int init;           // INIT_*
+};
+
+// A checkpoint tensor: the slot it lives in.  gate_proj and up_proj are the halves of the GU-interleaved wgu (128 gate rows,
+// then the 128 up rows of the same features, ...); GLM's fused gate_up_proj holds all gate rows, then all up rows.
+enum { GU_GATE = 1, GU_UP = 2, GU_BOTH = 3 };
+struct WeightName {
+  const char* key;     // a layer's: matched in the name after "layers.N.", a global's: anywhere; no key contains another
+  const char* hf;      // globals: the checkpoint name (a layer's is "model.layers.N." + key)
+  int slot;            // row of lslots / gslots
+  int64_t off;         // element offset inside the slot (GU rows: 0)
+  int64_t rows, cols;  // HF shape; a vector is [rows, 1]
+  int gu;              // GU_*: which halves of wgu the tensor holds; 0: a plain copy at off
+};
+
 // activation layouts (dtx_train_cfg.recompute): every layer keeps its own saved set, or all layers share one that the
 // backward pass refills by re-running each layer's forward
 enum { KEEP_ALL = 1, RECOMPUTE_LAYER = 2 };
@@ -237,22 +267,21 @@ struct dtx_trainer {
   int32_t* d_row_valid = nullptr; // [micro_batch] per-row valid-token count
   double* d_host_red = nullptr;   // staging for dtx_allreduce_host
   int window = 0;                 // sliding-window attention span (0 = plain causal)
+  bool rope_glm = false;          // GLM's partial interleaved rotary: rope_cs / rope_cs_t hold head_dim / 4 frequencies
+  // base weights: the slot tables of a layer block and of the globals block (see Slot), the elements they add up to, and the
+  // checkpoint names that load into them
+  std::vector<Slot<Layer>> lslots;
+  std::vector<Slot<dtx_trainer>> gslots;
+  int64_t layer_used = 0, glob_used = 0;
+  std::vector<WeightName> lnames, gnames;
   // ---- full-parameter SFT (train.full_finetune): every weight trains, no adapters (BASELINE.json configs[3]) ----
-  // Weights live in ONE flat bf16 buffer - L layer blocks [wqkv | wo | wgu | wdown | norm1 | norm2] then a globals block
-  // [embed | lm_head | final norm], each padded to a multiple of world * 128 elements - with a gradient buffer of the same
-  // layout.  Rank r owns elements [r, r + 1) * block / world of every block: the block's bf16 gradients are reduce-scattered
-  // in place (NCCL, on a side stream, as soon as the backward pass has finished the layer), the fp32 master weights and Adam
-  // moments exist for the owned slices only (ZeRO-1 style), and the updated bf16 slices are all-gathered in place.
+  // Weights live in ONE flat bf16 buffer - L layer blocks laid out by lslots, then a globals block laid out by gslots, each
+  // padded to a multiple of world * 128 elements - with a gradient buffer of the same layout.  Rank r owns elements
+  // [r, r + 1) * block / world of every block: the block's bf16 gradients are reduce-scattered in place (NCCL, on a side
+  // stream, as soon as the backward pass has finished the layer), the fp32 master weights and Adam moments exist for the
+  // owned slices only (ZeRO-1 style), and the updated bf16 slices are all-gathered in place.
   bool full = false;
-  bool qkv_bias = false;        // q|k|v biases (Qwen2): Layer::bias; full-parameter SFT keeps them at off_bias of the layer block
-  int64_t off_bias = 0;
-  bool qk_norm = false;         // q/k RMSNorm (Qwen3): Layer::qkn, Layer::qk_pre; full-parameter SFT keeps the weights at off_qkn
-  bool rope_glm = false;        // GLM's partial interleaved rotary: rope_cs / rope_cs_t hold head_dim / 4 frequencies
-  bool post_norms = false;      // Glm4's post-sublayer norms: Layer::pn, o_pre, down_pre; full-parameter SFT keeps pn at off_pn
-  int64_t off_pn = 0;
-  int64_t off_qkn = 0;
   int64_t layer_elems = 0, glob_elems = 0;
-  int64_t off_wo = 0, off_wgu = 0, off_wdown = 0, off_n1 = 0, off_n2 = 0, goff_lm = 0, goff_nf = 0, layer_used = 0, glob_used = 0;
   bf16 *w_flat = nullptr, *g_flat = nullptr;
   float *master = nullptr, *fm = nullptr, *fv = nullptr, *embed_g32 = nullptr, *ndw_scratch = nullptr;
   bool master_valid = false;
@@ -274,12 +303,9 @@ struct dtx_trainer {
   float2* rope_cs_t = nullptr;  // the same table transposed to [D/2][S]: coalesced when thread r needs position q0 + r (attention backward epilogues)
   int split_b = 1, split_a = 1;
 
-  // which base tensors have been uploaded: [0] embed, [1] lm_head, [2] final norm, then 9 per layer
-  // (q, k, v, o, gate, up, down, norm1, norm2); a step with a hole in this map would train on uninitialised memory
+  // which base tensors have been uploaded: one flag per row of gnames, then one per row of lnames for every layer; a step with a
+  // hole in this map would train on uninitialised memory
   std::vector<uint8_t> loaded;
-  std::vector<uint8_t> bias_loaded;  // qkv_bias: q, k, v bias of every layer
-  std::vector<uint8_t> qkn_loaded;   // qk_norm: q_norm, k_norm weight of every layer
-  std::vector<uint8_t> pn_loaded;    // post_norms: post_self_attn_layernorm, post_mlp_layernorm weight of every layer
   bool all_random = false;
   bool have_lora = false;
   cudaEvent_t ev_fb = nullptr, ev_ar = nullptr;
@@ -334,33 +360,23 @@ struct dtx_trainer {
   cudaError_t zero(T* p, size_t n) {
     return dry ? cudaSuccess : cudaMemset(p, 0, n * sizeof(T));
   }
+  // full-parameter SFT: the gradient of weight element `w` (same layout as the weights)
+  bf16* grad_of(const bf16* w) const { return g_flat + (w - w_flat); }
   // first base tensor that has not been loaded, or nullptr when the model is complete
   const char* missing_weight(char* buf, size_t n) const {
     if (all_random) return nullptr;
-    static const char* top[3] = {"model.embed_tokens.weight", "lm_head.weight", "model.norm.weight"};
-    static const char* per[9] = {"self_attn.q_proj", "self_attn.k_proj", "self_attn.v_proj", "self_attn.o_proj", "mlp.gate_proj",
-                                 "mlp.up_proj", "mlp.down_proj", "input_layernorm", "post_attention_layernorm"};
-    for (size_t i = 0; i < loaded.size(); ++i)
-      if (!loaded[i]) {
-        if (i < 3) snprintf(buf, n, "%s", top[i]);
-        else snprintf(buf, n, "model.layers.%zu.%s.weight", (i - 3) / 9, per[(i - 3) % 9]);
+    const size_t G = gnames.size(), K = lnames.size();
+    for (size_t i = 0; i < loaded.size(); ++i) {
+      if (loaded[i]) continue;
+      if (i < G) {
+        snprintf(buf, n, "%s", gnames[i].hf);
         return buf;
       }
-    for (size_t i = 0; i < bias_loaded.size(); ++i)
-      if (!bias_loaded[i]) {
-        snprintf(buf, n, "model.layers.%zu.%s.bias", i / 3, per[i % 3]);
-        return buf;
-      }
-    for (size_t i = 0; i < qkn_loaded.size(); ++i)
-      if (!qkn_loaded[i]) {
-        snprintf(buf, n, "model.layers.%zu.self_attn.%s.weight", i / 2, i % 2 ? "k_norm" : "q_norm");
-        return buf;
-      }
-    for (size_t i = 0; i < pn_loaded.size(); ++i)
-      if (!pn_loaded[i]) {
-        snprintf(buf, n, "model.layers.%zu.%s.weight", i / 2, i % 2 ? "post_mlp_layernorm" : "post_self_attn_layernorm");
-        return buf;
-      }
+      const WeightName& w = lnames[(i - G) % K];
+      if (w.gu == GU_BOTH) continue;  // a second name for the gate and up rows, which have flags of their own
+      snprintf(buf, n, "model.layers.%zu.%s", (i - G) / K, w.key);
+      return buf;
+    }
     return nullptr;
   }
 };
@@ -451,35 +467,14 @@ int create_buffers(dtx_trainer* t) {
   const dtx_model_cfg& mc = t->mc;
   const dtx_train_cfg& tc = t->tc;
   const size_t d = mc.hidden, F = mc.ffn, V = mc.vocab, L = mc.n_layers, M = t->M, RP = t->RP, W = t->W, KA = t->KA;
-  const size_t dq = t->dq, QK = t->dq + t->dkv, NQK = 2 * mc.head_dim;  // attention width, q|k width, q_norm | k_norm
+  const size_t dq = t->dq, QK = t->dq + t->dkv;  // attention width, q|k width
   bool ok = true;
   const bool full = t->full;
   if (full) {
     // one flat weight buffer + one flat gradient buffer; every block padded so that it splits evenly over the ranks
     const size_t unit = static_cast<size_t>(t->world) * 128;
     auto pad = [&](size_t n) { return (n + unit - 1) / unit * unit; };
-    t->off_wo = W * d;
-    t->off_wgu = t->off_wo + d * dq;
-    t->off_wdown = t->off_wgu + 2 * F * d;
-    t->off_n1 = t->off_wdown + d * F;
-    t->off_n2 = t->off_n1 + d;
-    t->layer_used = t->off_n2 + d;
-    if (t->qkv_bias) {  // no weight decay either (HF get_decay_parameter_names excludes "bias"): inside the block's no-decay tail
-      t->off_bias = t->layer_used;
-      t->layer_used += W;
-    }
-    if (t->qk_norm) {  // the same for the q/k norm weights (HF excludes "_norm." names from weight decay)
-      t->off_qkn = t->layer_used;
-      t->layer_used += NQK;
-    }
-    if (t->post_norms) {  // and for the post-sublayer norm weights ("layernorm" names)
-      t->off_pn = t->layer_used;
-      t->layer_used += 2 * d;
-    }
     t->layer_elems = pad(t->layer_used);
-    t->goff_lm = V * d;
-    t->goff_nf = 2 * V * d;
-    t->glob_used = 2 * V * d + d;
     t->glob_elems = pad(t->glob_used);
     const size_t total = L * t->layer_elems + t->glob_elems, shard = total / t->world;
     ok = ok && t->alloc(&t->w_flat, total) && t->alloc(&t->g_flat, total);
@@ -491,46 +486,29 @@ int create_buffers(dtx_trainer* t) {
     CKM(t->zero(t->fm, shard));
     CKM(t->zero(t->fv, shard));
     bf16* gl = t->w_flat + L * t->layer_elems;
-    t->embed = gl;
-    t->lm_head = gl + t->goff_lm;
-    t->normf = gl + t->goff_nf;
+    for (const auto& s : t->gslots) t->*s.mem = gl + s.off;
     t->n_train = static_cast<int64_t>(L * t->layer_used + t->glob_used);
   } else {
-    ok = ok && t->alloc(&t->embed, V * d) && t->alloc(&t->lm_head, V * d) && t->alloc(&t->normf, d);
+    for (const auto& s : t->gslots) ok = ok && t->alloc(&(t->*s.mem), s.n);
     ok = ok && t->alloc(&t->a_cat_all, L * RP * KA) && t->alloc(&t->b_ext_all, L * W * RP);
     if (!ok) return DTX_ERR_CUDA;
     CKM(t->zero(t->a_cat_all, L * RP * KA));
     CKM(t->zero(t->b_ext_all, L * W * RP));
   }
-  t->base_bytes = static_cast<int64_t>((2 * V * d + d) * sizeof(bf16));
-  t->loaded.assign(3 + 9 * L, 0);
-  t->bias_loaded.assign(t->qkv_bias ? 3 * L : 0, 0);
-  t->qkn_loaded.assign(t->qk_norm ? 2 * L : 0, 0);
-  t->pn_loaded.assign(t->post_norms ? 2 * L : 0, 0);
+  t->base_bytes = static_cast<int64_t>((t->glob_used + L * t->layer_used) * sizeof(bf16));
+  t->loaded.assign(t->gnames.size() + L * t->lnames.size(), 0);
   t->layers.resize(L);
   t->xs.resize(L + 1);
   for (size_t l = 0; l <= L; ++l) ok = ok && t->alloc(&t->xs[l], M * d);
   for (size_t l = 0; l < L && ok; ++l) {
     Layer& y = t->layers[l];
     if (full) {
-      bf16* blk = t->w_flat + l * t->layer_elems;
-      y.wqkv = blk; y.wo = blk + t->off_wo; y.wgu = blk + t->off_wgu; y.wdown = blk + t->off_wdown;
-      y.norm1 = blk + t->off_n1; y.norm2 = blk + t->off_n2;
-      if (t->qkv_bias) y.bias = blk + t->off_bias;
-      if (t->qk_norm) y.qkn = blk + t->off_qkn;
-      if (t->post_norms) y.pn = blk + t->off_pn;
+      for (const auto& s : t->lslots) y.*s.mem = t->w_flat + l * t->layer_elems + s.off;
     } else {
-      ok = ok && t->alloc(&y.wqkv, W * d) && t->alloc(&y.wo, d * dq) && t->alloc(&y.wgu, 2 * F * d) &&
-           t->alloc(&y.wdown, d * F) && t->alloc(&y.norm1, d) && t->alloc(&y.norm2, d);
-      if (t->qkv_bias) ok = ok && t->alloc(&y.bias, W);
-      if (t->qk_norm) ok = ok && t->alloc(&y.qkn, NQK);
-      if (t->post_norms) ok = ok && t->alloc(&y.pn, 2 * d);
+      for (const auto& s : t->lslots) ok = ok && t->alloc(&(y.*s.mem), s.n);
       y.a_cat = t->a_cat_all + l * RP * KA;
       y.b_ext = t->b_ext_all + l * W * RP;
     }
-    t->base_bytes +=
-        static_cast<int64_t>((W * d + d * dq + 3 * F * d + 2 * d + (t->qkv_bias ? W : 0) + (t->qk_norm ? NQK : 0) +
-                              (t->post_norms ? 2 * d : 0)) * sizeof(bf16));
     if (t->recompute == RECOMPUTE_LAYER && l > 0) {  // one saved set, refilled layer by layer
       const Layer& y0 = t->layers[0];
       y.h1 = y0.h1; y.t = y0.t; y.hd = y0.hd; y.qkv = y0.qkv; y.attn = y0.attn; y.x_mid = y0.x_mid; y.gu = y0.gu;
@@ -542,8 +520,8 @@ int create_buffers(dtx_trainer* t) {
     if (!full) ok = ok && t->alloc(&y.t, M * RP);
     ok = ok && t->alloc(&y.h1, M * d) && t->alloc(&y.qkv, M * W) &&
          t->alloc(&y.attn, M * dq) && t->alloc(&y.x_mid, M * d) && t->alloc(&y.gu, M * 2 * F);
-    if (t->qk_norm) ok = ok && t->alloc(&y.qk_pre, M * QK);
-    if (t->post_norms)
+    if (t->ext.qk_norm) ok = ok && t->alloc(&y.qk_pre, M * QK);
+    if (t->ext.post_norms)
       ok = ok && t->alloc(&y.o_pre, M * d) && t->alloc(&y.down_pre, M * d) && t->alloc(&y.rstd_pn1, M) && t->alloc(&y.rstd_pn2, M);
     if (t->dropout) ok = ok && t->alloc(&y.hd, M * KA);
     ok = ok && t->alloc(&y.lse, static_cast<size_t>(tc.micro_batch) * mc.n_heads * tc.seq_len) && t->alloc(&y.rstd1, M) &&
@@ -637,9 +615,8 @@ int refresh_shadows(dtx_trainer* t) {
 // CTAs and use HBM bandwidth the tensor-bound GEMM leaves idle, so that the expansion disappears from the critical path.
 int nf4_expand(dtx_trainer* t, int l, int which, cudaStream_t s) {
   Layer& y = t->layers[l];
-  const int64_t d = t->mc.hidden, F = t->mc.ffn;
-  const int64_t n[4] = {static_cast<int64_t>(t->W) * d, d * t->dq, 2 * F * d, d * F};
-  CK(nf4_dequant_bf16(y.q4[which], y.absmax[which], t->scratch_w[which], n[which], s), 1);
+  for (const auto& sl : t->lslots)
+    if (sl.nf4 == which) CK(nf4_dequant_bf16(y.q4[which], y.absmax[which], t->scratch_w[which], sl.n, s), 1);
   return DTX_OK;
 }
 // next (layer, matrix) the step will ask for after (l, which) in `phase` (PH_*), when it can be expanded ahead: always a
@@ -899,9 +876,8 @@ int fwd_bwd(dtx_trainer* t, bool backward) {
     g.epilogue = accumulate ? EPI_BF16_ADD : EPI_BF16; g.R = accumulate ? dW : nullptr; g.ldr = n_in;
     return gemm_bf16(g, s);
   };
-  bf16* gglob = t->full ? t->g_flat + static_cast<int64_t>(L) * t->layer_elems : nullptr;
   if (t->full) {  // lm_head weight gradient (h2 still holds the final-norm output) and the final norm's weight gradient
-    CK(dw_gemm(t->dlogits, V, t->h2, d, gglob + t->goff_lm), 1);
+    CK(dw_gemm(t->dlogits, V, t->h2, d, t->grad_of(t->lm_head)), 1);
   }
   {  // d h_f = dlogits * W_lm  (compact rows in LoRA mode)
     GemmArgs g;
@@ -909,7 +885,7 @@ int fwd_bwd(dtx_trainer* t, bool backward) {
     g.M = M; g.N = d; g.K = V; g.epilogue = EPI_BF16; g.m_eff = m_eff;
     CK(gemm_bf16(g, s), 1);
   }
-  if (t->full) CK(rmsnorm_dw(t->dh, t->xs[L], t->rstdf, M, d, t->ndw_scratch, gglob + t->goff_nf, accumulate, s), 2);
+  if (t->full) CK(rmsnorm_dw(t->dh, t->xs[L], t->rstdf, M, d, t->ndw_scratch, t->grad_of(t->normf), accumulate, s), 2);
   CK(rmsnorm_bwd(t->dh, t->xs[L], t->normf, t->rstdf, nullptr, t->dx_a, M, d, s, row_map), 1);
   bf16* cur = t->dx_a;
   bf16* other = t->dx_b;
@@ -919,16 +895,15 @@ int fwd_bwd(dtx_trainer* t, bool backward) {
       if (rc) return rc;
     }
     Layer& y = t->layers[l];
-    bf16* gl_w = t->full ? t->g_flat + static_cast<int64_t>(l) * t->layer_elems : nullptr;  // this layer's gradient block
     const bf16* d_down = cur;  // gradient of the down-projection output
     if (y.pn) {  // through post_mlp_layernorm: d down_pre into dh (free until the dh2 GEMM below); full SFT: its weight gradient
-      if (t->full) CK(rmsnorm_dw(cur, y.down_pre, y.rstd_pn2, M, d, t->ndw_scratch, gl_w + t->off_pn + d, accumulate, s), 2);
+      if (t->full) CK(rmsnorm_dw(cur, y.down_pre, y.rstd_pn2, M, d, t->ndw_scratch, t->grad_of(y.pn + d), accumulate, s), 2);
       CK(rmsnorm_bwd(cur, y.down_pre, y.pn + d, y.rstd_pn2, nullptr, t->dh, M, d, s), 1);
       d_down = t->dh;
     }
     if (t->full) {  // dWdown = d x_out^T * act: act = silu(gate) * up is recomputed from the saved gate|up (one HBM-bound pass)
       CK(swiglu_fwd(y.gu, t->act, M, F, 1, s), 1);
-      CK(dw_gemm(d_down, d, t->act, F, gl_w + t->off_wdown), 1);
+      CK(dw_gemm(d_down, d, t->act, F, t->grad_of(y.wdown)), 1);
     }
     {  // dact = dx * Wdown ; fused: d[gate|up] straight from the accumulator, dact never touches HBM
       BASEW(W_DOWN, wdown);
@@ -950,13 +925,13 @@ int fwd_bwd(dtx_trainer* t, bool backward) {
     }
     if (t->full) {  // dWgu = d[gate|up]^T * h2 (h2 = norm2(x_mid) recomputed) and the norm's own weight gradient
       CK(rmsnorm_fwd(y.x_mid, y.norm2, t->h2, nullptr, M, d, mc.rms_eps, s), 1);
-      CK(dw_gemm(t->dgu, 2 * F, t->h2, d, gl_w + t->off_wgu), 1);
-      CK(rmsnorm_dw(t->dh, y.x_mid, y.rstd2, M, d, t->ndw_scratch, gl_w + t->off_n2, accumulate, s), 2);
+      CK(dw_gemm(t->dgu, 2 * F, t->h2, d, t->grad_of(y.wgu)), 1);
+      CK(rmsnorm_dw(t->dh, y.x_mid, y.rstd2, M, d, t->ndw_scratch, t->grad_of(y.norm2), accumulate, s), 2);
     }
     CK(rmsnorm_bwd(t->dh, y.x_mid, y.norm2, y.rstd2, cur, other, M, d, s), 1);  // other = d x_mid
     const bf16* d_o = other;  // gradient of the o-projection output
     if (y.pn) {  // through post_self_attn_layernorm: d o_pre into dh (free until the dh1 GEMM below)
-      if (t->full) CK(rmsnorm_dw(other, y.o_pre, y.rstd_pn1, M, d, t->ndw_scratch, gl_w + t->off_pn, accumulate, s), 2);
+      if (t->full) CK(rmsnorm_dw(other, y.o_pre, y.rstd_pn1, M, d, t->ndw_scratch, t->grad_of(y.pn), accumulate, s), 2);
       CK(rmsnorm_bwd(other, y.o_pre, y.pn, y.rstd_pn1, nullptr, t->dh, M, d, s), 1);
       d_o = t->dh;
     }
@@ -967,7 +942,7 @@ int fwd_bwd(dtx_trainer* t, bool backward) {
       g.M = M; g.N = dq; g.K = d; g.epilogue = EPI_BF16;
       CK(gemm_bf16(g, s), 1);
     }
-    if (t->full) CK(dw_gemm(d_o, d, y.attn, dq, gl_w + t->off_wo), 1);  // dWo = d x_mid^T * attn
+    if (t->full) CK(dw_gemm(d_o, d, y.attn, dq, t->grad_of(y.wo)), 1);  // dWo = d x_mid^T * attn
     {
       AttnArgs a;
       a.qkv = y.qkv; a.out = y.attn; a.lse = y.lse; a.B = B; a.S = S; a.H = H; a.Hkv = Hkv; a.scale = att_scale;
@@ -987,7 +962,7 @@ int fwd_bwd(dtx_trainer* t, bool backward) {
     if (y.qkn) {  // through the q/k norm (Qwen3), in place on the q|k columns of dqkv; full-parameter SFT: d q_norm | d k_norm
       // the dw partials: at most as many 256-float blocks as ndw_scratch (64 * d floats) holds
       const int nblk = std::min(QKN_MAX_BLOCKS, 64 * d / 256);
-      CK(qk_norm_bwd(t->dqkv, W, y.qk_pre, QK, M, dq, QK, y.qkn, y.qkn + D, mc.rms_eps, t->full ? gl_w + t->off_qkn : nullptr,
+      CK(qk_norm_bwd(t->dqkv, W, y.qk_pre, QK, M, dq, QK, y.qkn, y.qkn + D, mc.rms_eps, t->full ? t->grad_of(y.qkn) : nullptr,
                      t->ndw_scratch, nblk, accumulate, s), t->full ? 2 : 1);
     }
     if (lora) {  // dt = dqkv * B_ext   [M, RP]
@@ -996,8 +971,8 @@ int fwd_bwd(dtx_trainer* t, bool backward) {
       g.M = M; g.N = RP; g.K = W; g.epilogue = EPI_BF16; g.block_n = 64;
       CK(gemm_bf16(g, s), 1);
     }
-    if (t->full) CK(dw_gemm(t->dqkv, W, y.h1, d, gl_w), 1);  // dWqkv = dqkv^T * h1 (dqkv already carries the inverse rotary)
-    if (t->full && t->qkv_bias) CK(bias_grad(t->dqkv, W, M, W, gl_w + t->off_bias, accumulate, s), 1);  // db = column sums of dqkv
+    if (t->full) CK(dw_gemm(t->dqkv, W, y.h1, d, t->grad_of(y.wqkv)), 1);  // dWqkv = dqkv^T * h1 (dqkv already carries the inverse rotary)
+    if (t->full && y.bias) CK(bias_grad(t->dqkv, W, M, W, t->grad_of(y.bias), accumulate, s), 1);  // db = column sums of dqkv
     // LoRA: layer 0's input gradient has no consumer (the embedding is frozen, SURVEY §8a): its dh1 GEMM, the dropout-branch
     // gradient and the norm-1 backward are skipped.  Full-parameter SFT trains the embedding and needs them.
     const bool need_dx = l > 0 || t->full;
@@ -1044,10 +1019,10 @@ int fwd_bwd(dtx_trainer* t, bool backward) {
       CK(cudaGetLastError(), 2);
     }
     }  // lora
-    if (t->full) CK(rmsnorm_dw(t->dh, t->xs[l], y.rstd1, M, d, t->ndw_scratch, gl_w + t->off_n1, accumulate, s), 2);
+    if (t->full) CK(rmsnorm_dw(t->dh, t->xs[l], y.rstd1, M, d, t->ndw_scratch, t->grad_of(y.norm1), accumulate, s), 2);
     if (need_dx) CK(rmsnorm_bwd(t->dh, t->xs[l], y.norm1, y.rstd1, other, cur, M, d, s), 1);  // cur = d x_in
     if (t->full && t->rs_now && t->world > 1) {  // this layer's gradients are final: reduce-scatter them while the backward pass goes on
-      int rc = reduce_scatter_block(t, gl_w, t->layer_elems, l);
+      int rc = reduce_scatter_block(t, t->g_flat + static_cast<int64_t>(l) * t->layer_elems, t->layer_elems, l);
       if (rc) return rc;
     }
   }
@@ -1055,7 +1030,7 @@ int fwd_bwd(dtx_trainer* t, bool backward) {
     const size_t vd = static_cast<size_t>(V) * d;
     CKM(cudaMemsetAsync(t->embed_g32, 0, vd * sizeof(float), s));
     CK(embedding_bwd(t->d_ids, cur, t->embed_g32, M, d, V, s), 1);
-    CK(add_f32_into_bf16(t->embed_g32, gglob, static_cast<int64_t>(vd), accumulate, s), 1);
+    CK(add_f32_into_bf16(t->embed_g32, t->grad_of(t->embed), static_cast<int64_t>(vd), accumulate, s), 1);
   }
   return DTX_OK;
 }
@@ -1091,9 +1066,16 @@ int optimizer_step(dtx_trainer* t, float* lr_used) {
   return DTX_OK;
 }
 
+template <class Owner>
+int64_t nodecay_from(const std::vector<Slot<Owner>>& slots, int64_t used) {
+  for (const auto& s : slots)
+    if (s.nodecay) return s.off;
+  return used;
+}
+
 // Full-parameter SFT: the blocks' bf16 gradients have been (or are now) reduce-scattered in place; every rank then runs
 // clip + AdamW on the slices it owns (fp32 master weights + moments, ZeRO-1 style) and the updated bf16 slices are
-// all-gathered in place.  HF's no-decay set (RMSNorm weights) sits at the end of every block.
+// all-gathered in place.  HF's no-decay set (norm weights, biases) sits at the end of every block.
 int optimizer_step_full(dtx_trainer* t, float* lr_used) {
   const dtx_train_cfg& tc = t->tc;
   cudaStream_t s = t->stream;
@@ -1142,14 +1124,15 @@ int optimizer_step_full(dtx_trainer* t, float* lr_used) {
   const double lam = dtx_lr_lambda(tc.sched, t->opt_step, tc.warmup_steps, tc.total_steps);
   const float lr = static_cast<float>(static_cast<double>(tc.lr) * lam);
   const int step1 = t->opt_step + 1;
+  // no weight decay from the first no-decay slot of a block on (its tail, see Slot)
+  const int64_t nd_layer = nodecay_from(t->lslots, t->layer_used), nd_glob = nodecay_from(t->gslots, t->glob_used);
   for (int blk = 0; blk <= L; ++blk) {
     int64_t n, moff;
     bf16* g = slice(blk, t->g_flat, &n, &moff);
     bf16* w = slice(blk, t->w_flat, &n, &moff);
     AdamWShardArgs a;
     a.master = t->master + moff; a.m = t->fm + moff; a.v = t->fv + moff; a.g = g; a.w = w; a.n = n;
-    // RMSNorm weights (no weight decay): the tail [off_n1, layer_used) of a layer block, [goff_nf, glob_used) of the globals
-    const int64_t nd_begin = blk < L ? t->off_n1 : t->goff_nf, first = static_cast<int64_t>(t->rank) * n;
+    const int64_t nd_begin = blk < L ? nd_layer : nd_glob, first = static_cast<int64_t>(t->rank) * n;
     a.nodecay_from = nd_begin - first < 0 ? 0 : nd_begin - first;
     a.lr = lr; a.beta1 = tc.beta1; a.beta2 = tc.beta2; a.eps = tc.eps; a.weight_decay = tc.weight_decay;
     a.bias1 = static_cast<float>(1.0 - pow(static_cast<double>(tc.beta1), step1));
@@ -1380,6 +1363,53 @@ bool parse_layer(const char* name, int* layer, const char** rest) {
   return true;
 }
 
+// The base tensor an HF checkpoint name refers to.  A layer's tensors match by substring of the part after "layers.N.", the
+// globals anywhere in the name - except the final norm, whose key every layer norm's name ends in: it only matches outside a layer.
+struct NamedWeight {
+  const std::vector<WeightName>* names;  // gnames or lnames
+  size_t row;                            // of `names`
+  uint8_t* loaded;                       // the block's part of the loaded map, indexed like `names`
+  bf16* slot;                            // the slot's first element in the weights (nullptr once NF4-packed)
+  bool nf4;                              // the slot is one dtx_quantize_base packs
+  const WeightName& w() const { return (*names)[row]; }
+};
+int find_weight(dtx_trainer* t, const char* name, NamedWeight* out) {
+  int layer = -1;
+  const char* rest = nullptr;
+  const bool in_layer = parse_layer(name, &layer, &rest);
+  for (size_t i = 0; i < t->gnames.size(); ++i) {
+    const auto& s = t->gslots[t->gnames[i].slot];
+    if (strstr(name, t->gnames[i].key) && !(in_layer && s.mem == &dtx_trainer::normf)) {
+      *out = {&t->gnames, i, t->loaded.data(), t->*s.mem, false};
+      return DTX_OK;
+    }
+  }
+  if (!in_layer) return t->fail(DTX_ERR_INVALID, "unknown tensor name %s", name);
+  if (layer < 0 || layer >= t->mc.n_layers) return t->fail(DTX_ERR_INVALID, "%s: layer out of range", name);
+  for (size_t i = 0; i < t->lnames.size(); ++i) {
+    if (!strstr(rest, t->lnames[i].key)) continue;
+    const auto& s = t->lslots[t->lnames[i].slot];
+    *out = {&t->lnames, i, t->loaded.data() + t->gnames.size() + layer * t->lnames.size(), t->layers[layer].*s.mem, s.nf4 >= 0};
+    return DTX_OK;
+  }
+  return t->fail(DTX_ERR_INVALID, "unknown tensor name %s", name);
+}
+
+// copies the halves of wgu named by `gu` (GU_*) between the GU-interleaved device rows and the HF rows on the host
+cudaError_t gu_copy(bf16* dev, bf16* host, int gu, int64_t F, int64_t d, cudaMemcpyKind kind, cudaStream_t s) {
+  for (int h = 0; h < 2; ++h) {
+    if (!(gu & (1 << h))) continue;
+    for (int64_t b = 0; b < F / 128; ++b) {
+      bf16* dv = dev + (b * 256 + h * 128) * d;
+      bf16* hs = host + ((gu == GU_BOTH ? h * F : 0) + b * 128) * d;
+      const size_t bytes = 128 * d * sizeof(bf16);
+      cudaError_t e = kind == cudaMemcpyHostToDevice ? cudaMemcpyAsync(dv, hs, bytes, kind, s) : cudaMemcpyAsync(hs, dv, bytes, kind, s);
+      if (e != cudaSuccess) return e;
+    }
+  }
+  return cudaSuccess;
+}
+
 void to_bf16_host(const void* src, int dtype, size_t n, std::vector<bf16>& out) {
   out.resize(n);
   if (dtype == DTX_BF16) {
@@ -1461,10 +1491,7 @@ int check_ext(const dtx_model_cfg* mc, const dtx_model_ext* ext) {
 void setup_dims(dtx_trainer* t, const dtx_model_cfg* mc, const dtx_model_ext* ext, const dtx_train_cfg* tc, int world) {
   t->mc = *mc;
   if (ext) t->ext = *ext;
-  t->qkv_bias = t->ext.qkv_bias != 0;
-  t->qk_norm = t->ext.qk_norm != 0;
   t->rope_glm = t->ext.rope_glm != 0;
-  t->post_norms = t->ext.post_norms != 0;
   t->tc = *tc;
   t->world = world;
   t->M = tc->micro_batch * tc->seq_len;
@@ -1498,6 +1525,53 @@ void setup_dims(dtx_trainer* t, const dtx_model_cfg* mc, const dtx_model_ext* ex
   // Mistral-style sliding window: only a different mask once the sequence is longer than the window
   // (transformers 4.34.0 _make_sliding_window_causal_mask: triu(diagonal=-sliding_window), i.e. query i sees keys i - sw .. i)
   t->window = (mc->sliding_window > 0 && tc->seq_len > mc->sliding_window + 1) ? mc->sliding_window : 0;
+
+  // the weight blocks (see Slot and WeightName)
+  const int64_t d = mc->hidden, F = mc->ffn, V = mc->vocab, D = mc->head_dim, W = t->W, dq = t->dq, dkv = t->dkv;
+  auto lslot = [&](bf16* Layer::*mem, int64_t n, bool nodecay, int nf4, int init) {
+    t->lslots.push_back({mem, n, t->layer_used, nodecay, nf4, init});
+    t->layer_used += n;
+    return static_cast<int>(t->lslots.size()) - 1;
+  };
+  auto lname = [&](const char* key, int slot, int64_t off, int64_t rows, int64_t cols, int gu = 0) {
+    t->lnames.push_back({key, nullptr, slot, off, rows, cols, gu});
+  };
+  const int qkv = lslot(&Layer::wqkv, W * d, false, W_QKV, INIT_NORMAL);
+  lname("self_attn.q_proj.weight", qkv, 0, dq, d);
+  lname("self_attn.k_proj.weight", qkv, dq * d, dkv, d);
+  lname("self_attn.v_proj.weight", qkv, (dq + dkv) * d, dkv, d);
+  lname("self_attn.o_proj.weight", lslot(&Layer::wo, d * dq, false, W_O, INIT_NORMAL), 0, d, dq);
+  const int gu = lslot(&Layer::wgu, 2 * F * d, false, W_GU, INIT_NORMAL);
+  lname("mlp.gate_proj.weight", gu, 0, F, d, GU_GATE);
+  lname("mlp.up_proj.weight", gu, 0, F, d, GU_UP);
+  lname("mlp.gate_up_proj.weight", gu, 0, 2 * F, d, GU_BOTH);  // GLM (modeling_glm GlmMLP: chunk(2))
+  lname("mlp.down_proj.weight", lslot(&Layer::wdown, d * F, false, W_DOWN, INIT_NORMAL), 0, d, F);
+  lname("input_layernorm.weight", lslot(&Layer::norm1, d, true, -1, INIT_ONE), 0, d, 1);
+  lname("post_attention_layernorm.weight", lslot(&Layer::norm2, d, true, -1, INIT_ONE), 0, d, 1);
+  if (t->ext.qkv_bias) {  // Qwen2, GLM: one [W] vector in the row order of wqkv
+    const int b = lslot(&Layer::bias, W, true, -1, INIT_ZERO);
+    lname("self_attn.q_proj.bias", b, 0, dq, 1);
+    lname("self_attn.k_proj.bias", b, dq, dkv, 1);
+    lname("self_attn.v_proj.bias", b, dq + dkv, dkv, 1);
+  }
+  if (t->ext.qk_norm) {  // Qwen3: q_norm | k_norm
+    const int q = lslot(&Layer::qkn, 2 * D, true, -1, INIT_ONE);
+    lname("self_attn.q_norm.weight", q, 0, D, 1);
+    lname("self_attn.k_norm.weight", q, D, D, 1);
+  }
+  if (t->ext.post_norms) {  // Glm4: post_self_attn_layernorm | post_mlp_layernorm
+    const int p = lslot(&Layer::pn, 2 * d, true, -1, INIT_ONE);
+    lname("post_self_attn_layernorm.weight", p, 0, d, 1);
+    lname("post_mlp_layernorm.weight", p, d, d, 1);
+  }
+  auto global = [&](bf16* dtx_trainer::*mem, const char* hf, const char* key, int64_t rows, int64_t cols, bool nodecay, int init) {
+    t->gnames.push_back({key, hf, static_cast<int>(t->gslots.size()), 0, rows, cols, 0});
+    t->gslots.push_back({mem, rows * cols, t->glob_used, nodecay, -1, init});
+    t->glob_used += rows * cols;
+  };
+  global(&dtx_trainer::embed, "model.embed_tokens.weight", "embed_tokens.weight", V, d, false, INIT_NORMAL);
+  global(&dtx_trainer::lm_head, "lm_head.weight", "lm_head.weight", V, d, false, INIT_NORMAL);
+  global(&dtx_trainer::normf, "model.norm.weight", "norm.weight", d, 1, true, INIT_ONE);
 }
 
 // device bytes create_buffers() allocates for this configuration and activation layout: the same function in a sizing run,
@@ -1715,41 +1789,14 @@ int32_t dtx_load_tensor(dtx_trainer* t, const char* name, const void* host, int3
   cudaSetDevice(t->device);
   wait_all_weights(t);      // full-parameter SFT: no all-gather may still be writing the weight buffer
   t->master_valid = false;  // ... and the fp32 master copies are rebuilt from the bf16 weights at the next step
-  const int64_t d = t->mc.hidden, F = t->mc.ffn, V = t->mc.vocab, r = t->tc.lora_r, dq = t->dq, dkv = t->dkv;
+  const int64_t d = t->mc.hidden, r = t->tc.lora_r;
   const int64_t rows = shape[0], cols = nd == 2 ? shape[1] : 1;
   auto expect = [&](int64_t er, int64_t ec) { return rows == er && cols == ec; };
-  auto upload = [&](bf16* dst, size_t n) -> int {
-    std::vector<bf16> tmp;
-    to_bf16_host(host, dtype, n, tmp);
-    cudaError_t e = upload_sync(dst, tmp.data(), n * sizeof(bf16), t->stream);
-    if (e != cudaSuccess) return t->fail(DTX_ERR_CUDA, "upload %s: %s", name, cudaGetErrorString(e));
-    return DTX_OK;
-  };
-  if (strstr(name, "embed_tokens.weight")) {
-    if (!expect(V, d)) return t->fail(DTX_ERR_INVALID, "%s: expected [%lld,%lld]", name, (long long)V, (long long)d);
-    t->loaded[0] = 1;
-    return upload(t->embed, V * d);
-  }
-  if (strstr(name, "lm_head.weight")) {
-    if (!expect(V, d)) return t->fail(DTX_ERR_INVALID, "%s: expected [%lld,%lld]", name, (long long)V, (long long)d);
-    t->loaded[1] = 1;
-    return upload(t->lm_head, V * d);
-  }
   int layer = -1;
   const char* rest = nullptr;
-  if (!parse_layer(name, &layer, &rest)) {
-    if (strstr(name, "norm.weight")) {  // model.norm.weight
-      if (rows != d) return t->fail(DTX_ERR_INVALID, "%s: expected [%lld]", name, (long long)d);
-      t->loaded[2] = 1;
-      return upload(t->normf, d);
-    }
-    return t->fail(DTX_ERR_INVALID, "unknown tensor name %s", name);
-  }
-  if (layer < 0 || layer >= t->mc.n_layers) return t->fail(DTX_ERR_INVALID, "%s: layer out of range", name);
-  Layer& y = t->layers[layer];
-  uint8_t* lmap = t->loaded.data() + 3 + 9 * static_cast<size_t>(layer);
-  const bool is_lora_a = strstr(rest, "lora_A") != nullptr, is_lora_b = strstr(rest, "lora_B") != nullptr;
-  if (is_lora_a || is_lora_b) {
+  if (parse_layer(name, &layer, &rest) && (strstr(rest, "lora_A") || strstr(rest, "lora_B"))) {
+    if (layer < 0 || layer >= t->mc.n_layers) return t->fail(DTX_ERR_INVALID, "%s: layer out of range", name);
+    const bool is_lora_a = strstr(rest, "lora_A") != nullptr;
     char which = 0;
     if (strstr(rest, "q_proj")) which = 'q';
     else if (strstr(rest, "k_proj")) which = 'k';
@@ -1777,82 +1824,23 @@ int32_t dtx_load_tensor(dtx_trainer* t, const char* name, const void* host, int3
     CKM(cudaStreamSynchronize(t->stream));
     return DTX_OK;
   }
-  {  // q|k|v biases [dq] / [dkv]: one [W] vector per layer in the row order of wqkv (bf16 also under NF4, like bitsandbytes)
-    static const char* keys[3] = {"self_attn.q_proj.bias", "self_attn.k_proj.bias", "self_attn.v_proj.bias"};
-    const int64_t row0[3] = {0, dq, dq + dkv}, n[3] = {dq, dkv, dkv};
-    for (int i = 0; i < 3; ++i) {
-      if (!strstr(rest, keys[i])) continue;
-      if (!t->qkv_bias) return t->fail(DTX_ERR_INVALID, "%s: this trainer was created without q/k/v biases (dtx_model_ext.qkv_bias)", name);
-      if (nd != 1 || rows != n[i]) return t->fail(DTX_ERR_INVALID, "%s: expected [%lld]", name, (long long)n[i]);
-      int rc = upload(y.bias + row0[i], n[i]);
-      if (rc == DTX_OK) t->bias_loaded[3 * static_cast<size_t>(layer) + i] = 1;
-      return rc;
-    }
-  }
-  for (int i = 0; i < 2; ++i) {  // q_norm / k_norm [head_dim]: one [2 * head_dim] vector per layer (bf16 also under NF4)
-    if (!strstr(rest, i ? "self_attn.k_norm.weight" : "self_attn.q_norm.weight")) continue;
-    if (!t->qk_norm) return t->fail(DTX_ERR_INVALID, "%s: this trainer was created without q/k norms (dtx_model_ext.qk_norm)", name);
-    const int64_t D = t->mc.head_dim;
-    if (nd != 1 || rows != D) return t->fail(DTX_ERR_INVALID, "%s: expected [%lld]", name, (long long)D);
-    int rc = upload(y.qkn + i * D, D);
-    if (rc == DTX_OK) t->qkn_loaded[2 * static_cast<size_t>(layer) + i] = 1;
-    return rc;
-  }
-  for (int i = 0; i < 2; ++i) {  // Glm4 post-sublayer norms [d]: one [2 * d] vector per layer (bf16 also under NF4)
-    if (!strstr(rest, i ? "post_mlp_layernorm.weight" : "post_self_attn_layernorm.weight")) continue;
-    if (!t->post_norms) return t->fail(DTX_ERR_INVALID, "%s: this trainer was created without post-sublayer norms (dtx_model_ext.post_norms)", name);
-    if (nd != 1 || rows != d) return t->fail(DTX_ERR_INVALID, "%s: expected [%lld]", name, (long long)d);
-    int rc = upload(y.pn + i * d, d);
-    if (rc == DTX_OK) t->pn_loaded[2 * static_cast<size_t>(layer) + i] = 1;
-    return rc;
-  }
-  if (t->quant4 && !strstr(rest, "layernorm"))
+  NamedWeight nw;
+  int rc = find_weight(t, name, &nw);
+  if (rc) return rc;
+  const WeightName& w = nw.w();
+  if (t->quant4 && nw.nf4)
     return t->fail(DTX_ERR_STATE, "%s: the base weights are already NF4-packed; load tensors before dtx_quantize_base", name);
-  // gate/up rows go to the GU-interleaved layout: 128 gate rows, then the 128 up rows of the same features, ...
-  if (strstr(rest, "mlp.gate_up_proj.weight")) {  // GLM's fused [gate F | up F] rows (modeling_glm GlmMLP: chunk(2))
-    if (!expect(2 * F, d)) return t->fail(DTX_ERR_INVALID, "%s: expected [%lld,%lld]", name, (long long)(2 * F), (long long)d);
-    std::vector<bf16> tmp;
-    to_bf16_host(host, dtype, static_cast<size_t>(2 * F) * d, tmp);
-    for (int which = 0; which < 2; ++which)
-      for (int64_t b = 0; b < F / 128; ++b) {
-        cudaError_t e = cudaMemcpyAsync(y.wgu + (b * 256 + which * 128) * d, tmp.data() + (which * F + b * 128) * d,
-                                        128 * d * sizeof(bf16), cudaMemcpyHostToDevice, t->stream);
-        if (e != cudaSuccess) return t->fail(DTX_ERR_CUDA, "upload %s: %s", name, cudaGetErrorString(e));
-      }
-    CKM(cudaStreamSynchronize(t->stream));  // `tmp` dies at the end of this scope
-    lmap[4] = lmap[5] = 1;
-    return DTX_OK;
-  }
-  for (int which = 0; which < 2; ++which) {
-    if (!strstr(rest, which ? "mlp.up_proj.weight" : "mlp.gate_proj.weight")) continue;
-    if (!expect(F, d)) return t->fail(DTX_ERR_INVALID, "%s: expected [%lld,%lld]", name, (long long)F, (long long)d);
-    std::vector<bf16> tmp;
-    to_bf16_host(host, dtype, static_cast<size_t>(F) * d, tmp);
-    for (int64_t b = 0; b < F / 128; ++b) {
-      cudaError_t e = cudaMemcpyAsync(y.wgu + (b * 256 + which * 128) * d, tmp.data() + b * 128 * d, 128 * d * sizeof(bf16),
-                                      cudaMemcpyHostToDevice, t->stream);
-      if (e != cudaSuccess) return t->fail(DTX_ERR_CUDA, "upload %s: %s", name, cudaGetErrorString(e));
-    }
-    CKM(cudaStreamSynchronize(t->stream));  // `tmp` dies at the end of this scope
-    lmap[4 + which] = 1;
-    return DTX_OK;
-  }
-  struct Slot { const char* key; bf16* dst; int64_t r, c; int bit; };
-  const Slot slots[] = {
-      {"self_attn.q_proj.weight", y.wqkv, dq, d, 0},                  {"self_attn.k_proj.weight", y.wqkv + dq * d, dkv, d, 1},
-      {"self_attn.v_proj.weight", y.wqkv + (dq + dkv) * d, dkv, d, 2}, {"self_attn.o_proj.weight", y.wo, d, dq, 3},
-      {"mlp.down_proj.weight", y.wdown, d, F, 6},             {"input_layernorm.weight", y.norm1, d, 1, 7},
-      {"post_attention_layernorm.weight", y.norm2, d, 1, 8},
-  };
-  for (const Slot& sl : slots) {
-    if (strstr(rest, sl.key)) {
-      if (!expect(sl.r, sl.c)) return t->fail(DTX_ERR_INVALID, "%s: expected [%lld,%lld]", name, (long long)sl.r, (long long)sl.c);
-      int rc = upload(sl.dst, sl.r * sl.c);
-      if (rc == DTX_OK) lmap[sl.bit] = 1;  // a step with a hole in this map is refused (check_ready)
-      return rc;
-    }
-  }
-  return t->fail(DTX_ERR_INVALID, "unknown tensor name %s", name);
+  if (!expect(w.rows, w.cols)) return t->fail(DTX_ERR_INVALID, "%s: expected [%lld,%lld]", name, (long long)w.rows, (long long)w.cols);
+  std::vector<bf16> tmp;
+  to_bf16_host(host, dtype, static_cast<size_t>(w.rows * w.cols), tmp);
+  cudaError_t e = w.gu ? gu_copy(nw.slot, tmp.data(), w.gu, t->mc.ffn, d, cudaMemcpyHostToDevice, t->stream)
+                       : cudaMemcpyAsync(nw.slot + w.off, tmp.data(), tmp.size() * sizeof(bf16), cudaMemcpyHostToDevice, t->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(t->stream);  // (see upload_sync)
+  if (e != cudaSuccess) return t->fail(DTX_ERR_CUDA, "upload %s: %s", name, cudaGetErrorString(e));
+  // a step with a hole in this map is refused (check_ready); GLM's gate_up_proj fills the gate_proj and up_proj rows
+  for (size_t j = 0; j < nw.names->size(); ++j)
+    if (j == nw.row || ((*nw.names)[j].gu & w.gu)) nw.loaded[j] = 1;
+  return DTX_OK;
 }
 
 int32_t dtx_init_random_weights(dtx_trainer* t, uint64_t seed) {
@@ -1860,29 +1848,18 @@ int32_t dtx_init_random_weights(dtx_trainer* t, uint64_t seed) {
   if (t->quant4) return t->fail(DTX_ERR_STATE, "init_random_weights: the base weights are already NF4-packed");
   t->master_valid = false;
   cudaSetDevice(t->device);
-  const int64_t d = t->mc.hidden, F = t->mc.ffn, V = t->mc.vocab;
   cudaStream_t s = t->stream;
   uint64_t k = seed * 1000003ull;
-  CK(fill_normal_bf16(t->embed, V * d, 0.02f, ++k, s), 1);
-  CK(fill_normal_bf16(t->lm_head, V * d, 0.02f, ++k, s), 1);
-  CK(fill_const_bf16(t->normf, d, 1.0f, s), 1);
-  for (Layer& y : t->layers) {
-    CK(fill_normal_bf16(y.wqkv, static_cast<int64_t>(t->W) * d, 0.02f, ++k, s), 1);
-    CK(fill_normal_bf16(y.wo, d * t->dq, 0.02f, ++k, s), 1);
-    CK(fill_normal_bf16(y.wgu, 2 * F * d, 0.02f, ++k, s), 1);
-    CK(fill_normal_bf16(y.wdown, d * F, 0.02f, ++k, s), 1);
-    CK(fill_const_bf16(y.norm1, d, 1.0f, s), 1);
-    CK(fill_const_bf16(y.norm2, d, 1.0f, s), 1);
-    if (y.bias) CK(fill_const_bf16(y.bias, t->W, 0.0f, s), 1);  // HF _init_weights zeroes Linear biases
-    if (y.qkn) CK(fill_const_bf16(y.qkn, 2 * t->mc.head_dim, 1.0f, s), 1);  // ... and sets RMSNorm weights to 1
-    if (y.pn) CK(fill_const_bf16(y.pn, 2 * d, 1.0f, s), 1);
-  }
+  // HF _init_weights: Linear and Embedding weights normal(0.02), Linear biases 0, RMSNorm weights 1
+  auto fill = [&](bf16* p, int64_t n, int init) {
+    return init == INIT_NORMAL ? fill_normal_bf16(p, n, 0.02f, ++k, s) : fill_const_bf16(p, n, init == INIT_ONE ? 1.0f : 0.0f, s);
+  };
+  for (const auto& sl : t->gslots) CK(fill(t->*sl.mem, sl.n, sl.init), 1);
+  for (Layer& y : t->layers)
+    for (const auto& sl : t->lslots) CK(fill(y.*sl.mem, sl.n, sl.init), 1);
   cudaError_t e = cudaStreamSynchronize(s);
   if (e != cudaSuccess) return t->fail(DTX_ERR_CUDA, "init_random_weights: %s", cudaGetErrorString(e));
   std::fill(t->loaded.begin(), t->loaded.end(), 1);
-  std::fill(t->bias_loaded.begin(), t->bias_loaded.end(), 1);
-  std::fill(t->qkn_loaded.begin(), t->qkn_loaded.end(), 1);
-  std::fill(t->pn_loaded.begin(), t->pn_loaded.end(), 1);
   return DTX_OK;
 }
 
@@ -1902,26 +1879,26 @@ int32_t dtx_quantize_base(dtx_trainer* t, int32_t mode) {
       return t->fail(DTX_ERR_STATE, "quantize_base: base weight %s is not loaded yet", m);
   }
   cudaSetDevice(t->device);
-  const int64_t d = t->mc.hidden, F = t->mc.ffn, W = t->W;
-  const int64_t n[4] = {W * d, d * t->dq, 2 * F * d, d * F};
-  for (int i = 0; i < 4; ++i)
-    if (n[i] % 64) return t->fail(DTX_ERR_INVALID, "quantize_base: matrix sizes must be multiples of the 64-element NF4 block");
+  for (const auto& sl : t->lslots)
+    if (sl.nf4 >= 0 && sl.n % 64) return t->fail(DTX_ERR_INVALID, "quantize_base: matrix sizes must be multiples of the 64-element NF4 block");
   cudaStream_t s = t->stream;
   for (Layer& y : t->layers) {
-    bf16** w[4] = {&y.wqkv, &y.wo, &y.wgu, &y.wdown};
-    for (int i = 0; i < 4; ++i) {
-      if (!t->alloc(&y.q4[i], static_cast<size_t>(n[i] / 2)) || !t->alloc(&y.absmax[i], static_cast<size_t>(n[i] / 64))) return DTX_ERR_CUDA;
-      CK(nf4_quantize_pack(*w[i], y.q4[i], y.absmax[i], n[i], s), 1);
+    for (const auto& sl : t->lslots) {
+      const int i = sl.nf4;
+      if (i < 0) continue;
+      if (!t->alloc(&y.q4[i], static_cast<size_t>(sl.n / 2)) || !t->alloc(&y.absmax[i], static_cast<size_t>(sl.n / 64))) return DTX_ERR_CUDA;
+      CK(nf4_quantize_pack(y.*sl.mem, y.q4[i], y.absmax[i], sl.n, s), 1);
     }
     CKM(cudaStreamSynchronize(s));
-    for (int i = 0; i < 4; ++i) {
-      t->release(*w[i], static_cast<size_t>(n[i]) * sizeof(bf16));
-      *w[i] = nullptr;
-      t->base_bytes += n[i] / 2 + (n[i] / 64) * 4 - n[i] * static_cast<int64_t>(sizeof(bf16));
+    for (const auto& sl : t->lslots) {
+      if (sl.nf4 < 0) continue;
+      t->release(y.*sl.mem, static_cast<size_t>(sl.n) * sizeof(bf16));
+      y.*sl.mem = nullptr;
+      t->base_bytes += sl.n / 2 + (sl.n / 64) * 4 - sl.n * static_cast<int64_t>(sizeof(bf16));
     }
   }
-  for (int i = 0; i < 4; ++i)
-    if (!t->alloc(&t->scratch_w[i], static_cast<size_t>(n[i]))) return DTX_ERR_CUDA;
+  for (const auto& sl : t->lslots)
+    if (sl.nf4 >= 0 && !t->alloc(&t->scratch_w[sl.nf4], static_cast<size_t>(sl.n))) return DTX_ERR_CUDA;
   if (g_nf4_prefetch) {
     CKM(cudaStreamCreateWithFlags(&t->copy_stream, cudaStreamNonBlocking));
     for (int i = 0; i < 4; ++i) {
@@ -2208,70 +2185,17 @@ int32_t dtx_export_weight(dtx_trainer* t, const char* name, void* host_out, int6
   cudaSetDevice(t->device);
   wait_all_weights(t);
   CKM(cudaStreamSynchronize(t->stream));
-  const int64_t d = t->mc.hidden, F = t->mc.ffn, V = t->mc.vocab, dq = t->dq, dkv = t->dkv, L = t->mc.n_layers;
-  const bf16* flat = grad ? t->g_flat : t->w_flat;
-  const bf16* gl = flat + L * t->layer_elems;
-  auto copy = [&](const bf16* src, int64_t n) -> int32_t {
-    if (nbytes < n * 2) return t->fail(DTX_ERR_INVALID, "%s: output buffer too small", name);
-    CKM(cudaMemcpyAsync(host_out, src, n * 2, cudaMemcpyDeviceToHost, t->stream));
-    CKM(cudaStreamSynchronize(t->stream));
-    return DTX_OK;
-  };
-  if (strstr(name, "embed_tokens.weight")) return copy(gl, V * d);
-  if (strstr(name, "lm_head.weight")) return copy(gl + t->goff_lm, V * d);
-  int layer = -1;
-  const char* rest = nullptr;
-  if (!parse_layer(name, &layer, &rest)) {
-    if (strstr(name, "norm.weight")) return copy(gl + t->goff_nf, d);
-    return t->fail(DTX_ERR_INVALID, "unknown tensor name %s", name);
-  }
-  if (layer < 0 || layer >= L) return t->fail(DTX_ERR_INVALID, "%s: layer out of range", name);
-  const bf16* blk = flat + layer * t->layer_elems;
-  if (strstr(rest, "mlp.gate_up_proj.weight")) {  // the fused HF tensor: all gate rows, then all up rows
-    if (nbytes < 2 * F * d * 2) return t->fail(DTX_ERR_INVALID, "%s: output buffer too small", name);
-    for (int which = 0; which < 2; ++which)
-      for (int64_t b = 0; b < F / 128; ++b)
-        CKM(cudaMemcpyAsync(static_cast<bf16*>(host_out) + (which * F + b * 128) * d, blk + t->off_wgu + (b * 256 + which * 128) * d,
-                            128 * d * 2, cudaMemcpyDeviceToHost, t->stream));
-    CKM(cudaStreamSynchronize(t->stream));
-    return DTX_OK;
-  }
-  for (int which = 0; which < 2; ++which) {
-    if (!strstr(rest, which ? "mlp.up_proj.weight" : "mlp.gate_proj.weight")) continue;
-    if (nbytes < F * d * 2) return t->fail(DTX_ERR_INVALID, "%s: output buffer too small", name);
-    for (int64_t b = 0; b < F / 128; ++b)
-      CKM(cudaMemcpyAsync(static_cast<bf16*>(host_out) + b * 128 * d, blk + t->off_wgu + (b * 256 + which * 128) * d, 128 * d * 2,
-                          cudaMemcpyDeviceToHost, t->stream));
-    CKM(cudaStreamSynchronize(t->stream));
-    return DTX_OK;
-  }
-  struct Slot { const char* key; int64_t off, n; };
-  const Slot slots[] = {
-      {"self_attn.q_proj.weight", 0, dq * d}, {"self_attn.k_proj.weight", dq * d, dkv * d},
-      {"self_attn.v_proj.weight", (dq + dkv) * d, dkv * d}, {"self_attn.o_proj.weight", t->off_wo, d * dq},
-      {"mlp.down_proj.weight", t->off_wdown, d * F}, {"input_layernorm.weight", t->off_n1, d},
-      {"post_attention_layernorm.weight", t->off_n2, d},
-  };
-  for (const Slot& sl : slots)
-    if (strstr(rest, sl.key)) return copy(blk + sl.off, sl.n);
-  if (t->qkv_bias) {
-    const Slot bias_slots[] = {
-        {"self_attn.q_proj.bias", t->off_bias, dq}, {"self_attn.k_proj.bias", t->off_bias + dq, dkv},
-        {"self_attn.v_proj.bias", t->off_bias + dq + dkv, dkv},
-    };
-    for (const Slot& sl : bias_slots)
-      if (strstr(rest, sl.key)) return copy(blk + sl.off, sl.n);
-  }
-  if (t->qk_norm) {
-    const int64_t D = t->mc.head_dim;
-    if (strstr(rest, "self_attn.q_norm.weight")) return copy(blk + t->off_qkn, D);
-    if (strstr(rest, "self_attn.k_norm.weight")) return copy(blk + t->off_qkn + D, D);
-  }
-  if (t->post_norms) {
-    if (strstr(rest, "post_self_attn_layernorm.weight")) return copy(blk + t->off_pn, d);
-    if (strstr(rest, "post_mlp_layernorm.weight")) return copy(blk + t->off_pn + d, d);
-  }
-  return t->fail(DTX_ERR_INVALID, "unknown tensor name %s", name);
+  NamedWeight nw;
+  int rc = find_weight(t, name, &nw);
+  if (rc) return rc;
+  const WeightName& w = nw.w();
+  if (nbytes < w.rows * w.cols * 2) return t->fail(DTX_ERR_INVALID, "%s: output buffer too small", name);
+  bf16* slot = grad ? t->grad_of(nw.slot) : nw.slot;
+  cudaError_t e = w.gu ? gu_copy(slot, static_cast<bf16*>(host_out), w.gu, t->mc.ffn, t->mc.hidden, cudaMemcpyDeviceToHost, t->stream)
+                       : cudaMemcpyAsync(host_out, slot + w.off, w.rows * w.cols * 2, cudaMemcpyDeviceToHost, t->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(t->stream);
+  if (e != cudaSuccess) return t->fail(DTX_ERR_CUDA, "export %s: %s", name, cudaGetErrorString(e));
+  return DTX_OK;
 }
 
 int64_t dtx_num_trainable(const dtx_trainer* t) { return t ? t->n_train : 0; }
