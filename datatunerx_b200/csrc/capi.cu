@@ -136,6 +136,7 @@ int32_t dtx_set_option(const char* name, int32_t value) {
     return DTX_OK;
   }
   if (strcmp(name, "varlen_split") == 0) {
+    if (value < 0 || value > 2) return DTX_ERR_INVALID;
     trainer_set_varlen_split(value);
     return DTX_OK;
   }

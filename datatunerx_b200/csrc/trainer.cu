@@ -261,7 +261,7 @@ struct dtx_trainer {
   int32_t *d_ids_full = nullptr, *d_labels_full = nullptr, *d_lens_full = nullptr;  // the whole ragged micro-batch (length groups gather from it)
   int32_t *d_pos = nullptr, *d_row_start = nullptr;  // packed batch: position of every row inside its sequence; first row of every sequence
   std::vector<int32_t> h_labels, h_lens;  // host copies of a device-resident ragged batch (the partition is planned on the host)
-  std::vector<float> h_row_sum;           // per-row evaluation statistics of the length groups, in group order
+  std::vector<float> h_row_sum;           // per-row evaluation statistics, rows in the order of the passes (RowStats)
   std::vector<int32_t> h_row_valid;
   float* d_row_sum = nullptr;     // [micro_batch] per-row summed token loss (evaluation)
   int32_t* d_row_valid = nullptr; // [micro_batch] per-row valid-token count
@@ -1173,7 +1173,6 @@ int set_batch_shape(dtx_trainer* t, int32_t seq_len_batch, bool have_lens) {
   t->cur_B = t->tc.micro_batch;
   t->cur_M = S * t->tc.micro_batch;
   t->use_seq_lens = have_lens;
-  t->packed = false;
   return DTX_OK;
 }
 
@@ -1197,7 +1196,7 @@ struct SubPlan {
 // PACKED layout of a ragged micro-batch (LoRA or full-parameter): sequence b gets its length rounded up to 128 rows, sequences back to back - one
 // pass over sum_b ceil128(len_b) rows instead of B * S_batch (or one pass per length group).  GEMMs, norms and CE simply see
 // fewer rows; the attention kernels take the first row of every sequence from a table; RoPE takes a row's position and the
-// label shift a sequence's end from a per-row position array.  Returns false when packing does not apply or saves nothing.
+// label shift a sequence's end from a per-row position array.
 // the layout alone (host arithmetic): first row of every sequence; true when it is smaller than the padded rectangle
 bool packed_rows(const int32_t* lens, int B, int S_batch, RowStarts* rs) {
   rs->n = B;
@@ -1207,12 +1206,6 @@ bool packed_rows(const int32_t* lens, int B, int S_batch, RowStarts* rs) {
     rs->start[b + 1] = rs->start[b] + std::min(S_batch, std::max(128, (len + 127) / 128 * 128));
   }
   return rs->start[B] < B * S_batch && rs->start[B] > 128;
-}
-bool plan_packed(const dtx_trainer* t, const int32_t* lens, int S_batch, RowStarts* rs) {
-  const int B = t->tc.micro_batch;
-  if (!g_varlen_pack || g_varlen_split == 0 || g_varlen_split == 2 || !lens || B < 1 || B > 64) return false;
-  if (!g_fused_epilogues || ((t->dq + t->dkv) % 256) || (t->W % 256)) return false;  // RoPE must run in the GEMM epilogue (per-row positions)
-  return packed_rows(lens, B, S_batch, rs);
 }
 
 struct PlanDims { int hidden, ffn, W, dq, n_sms, B; };  // what the cost model needs of the model / device / batch
@@ -1283,41 +1276,152 @@ int check_ready(dtx_trainer* t) {
   return DTX_OK;
 }
 
-// plan (optional, n > 1): run the micro-batch as length groups gathered from src_* (device, [micro_batch, S_src] / [micro_batch])
-int do_step(dtx_trainer* t, int32_t flags, float* loss_out, float* gnorm_out, float* lr_out, int32_t* stepped_out,
-            const SubPlan* plan = nullptr, const int32_t* src_ids = nullptr, const int32_t* src_labels = nullptr,
-            const int32_t* src_lens = nullptr, int S_src = 0) {
-  cudaEventRecord(t->ev0, t->stream);
-  const int accum = t->tc.grad_accum > 0 ? t->tc.grad_accum : 1;
-  t->rs_now = t->full && (t->micro_idx + 1 >= accum || (flags & DTX_STEP_FORCE));
-  int rc = DTX_OK;
-  t->last_groups = t->packed ? 0 : 1;
-  if (plan && plan->n > 1) {
-    t->last_groups = plan->n;
-    for (int g = 0; g < plan->n && rc == DTX_OK; ++g) {
+// One micro-batch as the caller hands it over: [micro_batch, S] ids and labels, optional true row lengths [micro_batch].
+struct BatchInput {
+  const int32_t *ids, *labels, *lens;  // lens null: every row is full
+  bool on_device;                      // device pointers (dtx_step_device), else host memory
+  int S;                               // seq_len_batch as set_batch_shape resolved it
+};
+
+// How a micro-batch runs: packed (one pass over rs), length groups (groups.n > 1) or one pass at the padded shape.
+struct BatchPlan {
+  bool packed = false;
+  RowStarts rs;
+  SubPlan groups;
+};
+
+// The layout decision for dtx_step, dtx_step_device and dtx_eval_loss alike.  A batch with row lengths is packed when that
+// is on, the fused RoPE epilogue applies (it takes per-row positions) and it saves rows; otherwise a LoRA batch runs as length
+// groups when the cost model cuts it.  Device input is planned on the host: the row lengths are read back once, and the
+// labels (B*S*4 bytes, for the groups' token count) only when grouping is planned - with the lengths when packing is off.
+int plan_batch(dtx_trainer* t, const BatchInput& in, BatchPlan* p) {
+  const int B = t->tc.micro_batch;
+  const size_t M = static_cast<size_t>(B) * in.S;
+  p->groups.n = 1;
+  const bool pack = in.lens && g_varlen_pack && g_varlen_split == 1 && B <= 64 && g_fused_epilogues && (t->dq + t->dkv) % 256 == 0 &&
+                    t->W % 256 == 0;
+  const bool group = in.lens && g_varlen_split && !t->full && B > 1 && B <= 64;
+  if (!pack && !group) return DTX_OK;
+  auto read_back = [&](const int32_t* src, std::vector<int32_t>& dst, size_t n) {
+    dst.resize(n);
+    return cudaMemcpyAsync(dst.data(), src, n * 4, cudaMemcpyDeviceToHost, t->stream);
+  };
+  const int32_t* lens = in.lens;
+  if (in.on_device) {
+    CKM(read_back(in.lens, t->h_lens, static_cast<size_t>(B)));
+    if (!pack) CKM(read_back(in.labels, t->h_labels, M));
+    CKM(cudaStreamSynchronize(t->stream));
+    lens = t->h_lens.data();
+  }
+  if (pack && packed_rows(lens, B, in.S, &p->rs)) {
+    p->packed = true;
+    return DTX_OK;
+  }
+  if (!group) return DTX_OK;
+  if (in.on_device && pack) {
+    CKM(read_back(in.labels, t->h_labels, M));
+    CKM(cudaStreamSynchronize(t->stream));
+  }
+  plan_groups(PlanDims{t->mc.hidden, t->mc.ffn, t->W, t->dq, t->n_sms, B}, lens, in.on_device ? t->h_labels.data() : in.labels, in.S,
+              &p->groups);
+  return DTX_OK;
+}
+
+// Per-row evaluation statistics (loss sum, labelled tokens) of the arrays the caller wants (either may be null).  run_batch
+// copies them pass by pass to h_row_sum / h_row_valid; once the stream is synchronised row k there is the caller's row order[k].
+struct RowStats {
+  float* sum;
+  int32_t* valid;
+  std::vector<int> order;
+};
+
+// Stage `in` as plan_batch lays it out and run its passes through fwd_bwd(t, backward).  The batch's cur_* / packed /
+// sub_accum / sub_ndiv are set here for each pass and put back to the whole micro-batch's on every exit.  A training step's
+// ev0 falls after the batch copies and pack_rows and before the groups' gathers.
+int run_batch(dtx_trainer* t, const BatchInput& in, bool backward, RowStats* stats = nullptr) {
+  BatchPlan p;
+  int rc = plan_batch(t, in, &p);
+  if (rc) return rc;
+  const int B = t->tc.micro_batch, S = in.S;
+  const size_t M = static_cast<size_t>(B) * S;
+  const bool grouped = p.groups.n > 1;
+  const cudaMemcpyKind kind = in.on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+  const int32_t *ids = in.ids, *labels = in.labels, *lens = in.lens;  // what pack_rows / gather_rows read
+  if (!p.packed && !grouped) {
+    CKM(cudaMemcpyAsync(t->d_ids, ids, M * 4, kind, t->stream));
+    CKM(cudaMemcpyAsync(t->d_labels, labels, M * 4, kind, t->stream));
+    if (lens) CKM(cudaMemcpyAsync(t->d_seq_lens, lens, static_cast<size_t>(B) * 4, kind, t->stream));
+  } else if (!in.on_device) {  // host input goes through the staging buffers
+    CKM(cudaMemcpyAsync(t->d_ids_full, ids, M * 4, kind, t->stream));
+    CKM(cudaMemcpyAsync(t->d_labels_full, labels, M * 4, kind, t->stream));
+    ids = t->d_ids_full;
+    labels = t->d_labels_full;
+    if (grouped) {
+      CKM(cudaMemcpyAsync(t->d_lens_full, lens, static_cast<size_t>(B) * 4, kind, t->stream));
+      lens = t->d_lens_full;
+    }
+  }
+  if (p.packed) {
+    CKM(cudaMemcpyAsync(t->d_seq_lens, in.lens, static_cast<size_t>(B) * 4, kind, t->stream));
+    CK(pack_rows(ids, labels, S, p.rs, t->d_ids, t->d_labels, t->d_pos, t->d_row_start, t->stream), 1);
+  }
+  if (backward) {
+    cudaEventRecord(t->ev0, t->stream);
+    t->last_groups = p.packed ? 0 : p.groups.n;
+  }
+  if (stats) {
+    t->h_row_sum.resize(static_cast<size_t>(B));
+    t->h_row_valid.resize(static_cast<size_t>(B));
+    stats->order.resize(static_cast<size_t>(B));
+    for (int k = 0; k < B; ++k) stats->order[k] = grouped ? p.groups.order[k] : k;
+  }
+  for (int g = 0; g < p.groups.n && rc == DTX_OK; ++g) {
+    int first = 0, rows = B, S_g = S;
+    if (grouped) {
       RowList rl;
-      rl.n = plan->start[g + 1] - plan->start[g];
-      for (int k = 0; k < rl.n; ++k) rl.rows[k] = plan->order[plan->start[g] + k];
-      cudaError_t ge = gather_rows(src_ids, src_labels, src_lens, S_src, rl, plan->S[g], t->d_ids, t->d_labels, t->d_seq_lens, t->stream);
-      if (ge != cudaSuccess) {
-        t->sub_accum = false;
-        t->sub_ndiv = 0;
-        return t->fail(DTX_ERR_CUDA, "gather_rows: %s", cudaGetErrorString(ge));
+      first = p.groups.start[g];
+      rows = rl.n = p.groups.start[g + 1] - first;
+      S_g = p.groups.S[g];
+      for (int k = 0; k < rows; ++k) rl.rows[k] = p.groups.order[first + k];
+      cudaError_t e = gather_rows(ids, labels, lens, S, rl, S_g, t->d_ids, t->d_labels, t->d_seq_lens, t->stream);
+      if (e != cudaSuccess) {
+        rc = t->fail(DTX_ERR_CUDA, "gather_rows: %s", cudaGetErrorString(e));
+        break;
       }
       t->launches += 1;
-      t->cur_B = rl.n;
-      t->cur_S = plan->S[g];
-      t->cur_M = rl.n * plan->S[g];
-      t->use_seq_lens = true;
-      t->sub_accum = g > 0;
-      t->sub_ndiv = plan->n_div;
-      rc = fwd_bwd(t, true);
     }
-    t->sub_accum = false;
-    t->sub_ndiv = 0;
-  } else {
-    rc = fwd_bwd(t, true);
+    t->cur_B = rows;
+    t->cur_S = S_g;
+    t->cur_M = p.packed ? p.rs.start[B] : rows * S_g;
+    t->packed = p.packed;
+    t->sub_accum = g > 0;
+    t->sub_ndiv = grouped ? p.groups.n_div : 0;
+    rc = fwd_bwd(t, backward);
+    if (rc == DTX_OK && stats) {
+      cudaError_t e = row_loss_stats(t->row_loss, t->d_shift, rows, S_g, t->d_row_sum, t->d_row_valid, t->stream,
+                                     p.packed ? t->d_row_start : nullptr);
+      // d_row_sum / d_row_valid are reused by the next group: these copies are stream-ordered in front of its kernels
+      if (e == cudaSuccess && stats->sum)
+        e = cudaMemcpyAsync(t->h_row_sum.data() + first, t->d_row_sum, static_cast<size_t>(rows) * 4, cudaMemcpyDeviceToHost, t->stream);
+      if (e == cudaSuccess && stats->valid)
+        e = cudaMemcpyAsync(t->h_row_valid.data() + first, t->d_row_valid, static_cast<size_t>(rows) * 4, cudaMemcpyDeviceToHost, t->stream);
+      if (e != cudaSuccess) rc = t->fail(DTX_ERR_CUDA, "eval row statistics: %s", cudaGetErrorString(e));
+      t->launches += 1;
+    }
   }
+  t->cur_B = B;
+  t->cur_S = S;
+  t->cur_M = static_cast<int>(M);
+  t->packed = t->sub_accum = false;
+  t->sub_ndiv = 0;
+  return rc;
+}
+
+// one training micro-batch: forward + backward, then the optimizer once grad_accum micro-batches (or DTX_STEP_FORCE) are in
+int do_step(dtx_trainer* t, const BatchInput& in, int32_t flags, float* loss_out, float* gnorm_out, float* lr_out, int32_t* stepped_out) {
+  const int accum = t->tc.grad_accum > 0 ? t->tc.grad_accum : 1;
+  t->rs_now = t->full && (t->micro_idx + 1 >= accum || (flags & DTX_STEP_FORCE));
+  int rc = run_batch(t, in, true);
   if (rc) return rc;
   cudaEventRecord(t->ev_fb, t->stream);
   t->micro_idx += 1;
@@ -1953,31 +2057,7 @@ int32_t dtx_step(dtx_trainer* t, const int32_t* ids, const int32_t* labels, cons
   int rc = check_ready(t);
   if (rc == DTX_OK) rc = set_batch_shape(t, seq_len_batch, seq_lens != nullptr);
   if (rc) return rc;
-  RowStarts rs;
-  if (plan_packed(t, seq_lens, t->cur_S, &rs)) {  // ragged batch, packed: staging buffers -> sequences back to back
-    CKM(cudaMemcpyAsync(t->d_ids_full, ids, static_cast<size_t>(t->cur_M) * 4, cudaMemcpyHostToDevice, t->stream));
-    CKM(cudaMemcpyAsync(t->d_labels_full, labels, static_cast<size_t>(t->cur_M) * 4, cudaMemcpyHostToDevice, t->stream));
-    CKM(cudaMemcpyAsync(t->d_seq_lens, seq_lens, static_cast<size_t>(t->tc.micro_batch) * 4, cudaMemcpyHostToDevice, t->stream));
-    CK(pack_rows(t->d_ids_full, t->d_labels_full, t->cur_S, rs, t->d_ids, t->d_labels, t->d_pos, t->d_row_start, t->stream), 1);
-    t->cur_M = rs.start[rs.n];
-    t->packed = true;
-    rc = do_step(t, flags, loss, gnorm, lr, stepped);
-    t->packed = false;
-    return rc;
-  }
-  SubPlan plan;
-  if (!t->full) plan_groups(PlanDims{t->mc.hidden, t->mc.ffn, t->W, t->dq, t->n_sms, t->tc.micro_batch}, seq_lens, labels, t->cur_S, &plan);
-  if (plan.n > 1) {  // ragged batch: the whole batch goes to the staging buffers, the length groups gather from there
-    const int S_src = t->cur_S;
-    CKM(cudaMemcpyAsync(t->d_ids_full, ids, static_cast<size_t>(t->cur_M) * 4, cudaMemcpyHostToDevice, t->stream));
-    CKM(cudaMemcpyAsync(t->d_labels_full, labels, static_cast<size_t>(t->cur_M) * 4, cudaMemcpyHostToDevice, t->stream));
-    CKM(cudaMemcpyAsync(t->d_lens_full, seq_lens, static_cast<size_t>(t->tc.micro_batch) * 4, cudaMemcpyHostToDevice, t->stream));
-    return do_step(t, flags, loss, gnorm, lr, stepped, &plan, t->d_ids_full, t->d_labels_full, t->d_lens_full, S_src);
-  }
-  CKM(cudaMemcpyAsync(t->d_ids, ids, static_cast<size_t>(t->cur_M) * 4, cudaMemcpyHostToDevice, t->stream));
-  CKM(cudaMemcpyAsync(t->d_labels, labels, static_cast<size_t>(t->cur_M) * 4, cudaMemcpyHostToDevice, t->stream));
-  if (seq_lens) CKM(cudaMemcpyAsync(t->d_seq_lens, seq_lens, static_cast<size_t>(t->tc.micro_batch) * 4, cudaMemcpyHostToDevice, t->stream));
-  return do_step(t, flags, loss, gnorm, lr, stepped);
+  return do_step(t, BatchInput{ids, labels, seq_lens, false, t->cur_S}, flags, loss, gnorm, lr, stepped);
 }
 
 int32_t dtx_step_device(dtx_trainer* t, const void* d_ids, const void* d_labels, const void* d_seq_lens, int32_t seq_len_batch,
@@ -1987,40 +2067,9 @@ int32_t dtx_step_device(dtx_trainer* t, const void* d_ids, const void* d_labels,
   int rc = check_ready(t);
   if (rc == DTX_OK) rc = set_batch_shape(t, seq_len_batch, d_seq_lens != nullptr);
   if (rc) return rc;
-  if (d_seq_lens && g_varlen_pack && g_varlen_split == 1 && t->tc.micro_batch <= 64) {
-    // the packed layout is planned on the host from the row lengths (B * 4 bytes)
-    t->h_lens.resize(static_cast<size_t>(t->tc.micro_batch));
-    CKM(cudaMemcpyAsync(t->h_lens.data(), d_seq_lens, t->h_lens.size() * 4, cudaMemcpyDeviceToHost, t->stream));
-    CKM(cudaStreamSynchronize(t->stream));
-    RowStarts rs;
-    if (plan_packed(t, t->h_lens.data(), t->cur_S, &rs)) {
-      CKM(cudaMemcpyAsync(t->d_seq_lens, d_seq_lens, static_cast<size_t>(t->tc.micro_batch) * 4, cudaMemcpyDeviceToDevice, t->stream));
-      CK(pack_rows(static_cast<const int32_t*>(d_ids), static_cast<const int32_t*>(d_labels), t->cur_S, rs, t->d_ids, t->d_labels, t->d_pos,
-                   t->d_row_start, t->stream), 1);
-      t->cur_M = rs.start[rs.n];
-      t->packed = true;
-      rc = do_step(t, flags, loss, gnorm, lr, stepped);
-      t->packed = false;
-      return rc;
-    }
-  }
-  if (d_seq_lens && g_varlen_split && !t->full && t->tc.micro_batch > 1 && t->tc.micro_batch <= 64) {
-    // the partition is planned on the host: fetch the row lengths and the labels (B*S*4 bytes, tens of microseconds)
-    t->h_lens.resize(static_cast<size_t>(t->tc.micro_batch));
-    t->h_labels.resize(static_cast<size_t>(t->cur_M));
-    CKM(cudaMemcpyAsync(t->h_lens.data(), d_seq_lens, t->h_lens.size() * 4, cudaMemcpyDeviceToHost, t->stream));
-    CKM(cudaMemcpyAsync(t->h_labels.data(), d_labels, t->h_labels.size() * 4, cudaMemcpyDeviceToHost, t->stream));
-    CKM(cudaStreamSynchronize(t->stream));
-    SubPlan plan;
-    plan_groups(PlanDims{t->mc.hidden, t->mc.ffn, t->W, t->dq, t->n_sms, t->tc.micro_batch}, t->h_lens.data(), t->h_labels.data(), t->cur_S, &plan);
-    if (plan.n > 1)
-      return do_step(t, flags, loss, gnorm, lr, stepped, &plan, static_cast<const int32_t*>(d_ids), static_cast<const int32_t*>(d_labels),
-                     static_cast<const int32_t*>(d_seq_lens), t->cur_S);
-  }
-  CKM(cudaMemcpyAsync(t->d_ids, d_ids, static_cast<size_t>(t->cur_M) * 4, cudaMemcpyDeviceToDevice, t->stream));
-  CKM(cudaMemcpyAsync(t->d_labels, d_labels, static_cast<size_t>(t->cur_M) * 4, cudaMemcpyDeviceToDevice, t->stream));
-  if (d_seq_lens) CKM(cudaMemcpyAsync(t->d_seq_lens, d_seq_lens, static_cast<size_t>(t->tc.micro_batch) * 4, cudaMemcpyDeviceToDevice, t->stream));
-  return do_step(t, flags, loss, gnorm, lr, stepped);
+  const BatchInput in{static_cast<const int32_t*>(d_ids), static_cast<const int32_t*>(d_labels), static_cast<const int32_t*>(d_seq_lens),
+                      true, t->cur_S};
+  return do_step(t, in, flags, loss, gnorm, lr, stepped);
 }
 
 int32_t dtx_eval_loss(dtx_trainer* t, const int32_t* ids, const int32_t* labels, const int32_t* seq_lens, int32_t seq_len_batch,
@@ -2030,92 +2079,18 @@ int32_t dtx_eval_loss(dtx_trainer* t, const int32_t* ids, const int32_t* labels,
   int rc = check_ready(t);
   if (rc == DTX_OK) rc = set_batch_shape(t, seq_len_batch, seq_lens != nullptr);
   if (rc) return rc;
-  const int B = t->tc.micro_batch;
-  float h = 0.f;
-  RowStarts rs;
-  if (plan_packed(t, seq_lens, t->cur_S, &rs)) {  // ragged batch, packed: one forward pass over the sequences back to back
-    CKM(cudaMemcpyAsync(t->d_ids_full, ids, static_cast<size_t>(t->cur_M) * 4, cudaMemcpyHostToDevice, t->stream));
-    CKM(cudaMemcpyAsync(t->d_labels_full, labels, static_cast<size_t>(t->cur_M) * 4, cudaMemcpyHostToDevice, t->stream));
-    CKM(cudaMemcpyAsync(t->d_seq_lens, seq_lens, static_cast<size_t>(B) * 4, cudaMemcpyHostToDevice, t->stream));
-    CK(pack_rows(t->d_ids_full, t->d_labels_full, t->cur_S, rs, t->d_ids, t->d_labels, t->d_pos, t->d_row_start, t->stream), 1);
-    t->cur_M = rs.start[rs.n];
-    t->packed = true;
-    rc = fwd_bwd(t, false);
-    t->packed = false;
-    if (rc) return rc;
-    CKM(cudaMemcpyAsync(&h, t->d_loss, 4, cudaMemcpyDeviceToHost, t->stream));
-    if (row_sum_out || row_valid_out) {
-      CK(row_loss_stats(t->row_loss, t->d_shift, B, t->cur_S, t->d_row_sum, t->d_row_valid, t->stream, t->d_row_start), 1);
-      if (row_sum_out) CKM(cudaMemcpyAsync(row_sum_out, t->d_row_sum, static_cast<size_t>(B) * 4, cudaMemcpyDeviceToHost, t->stream));
-      if (row_valid_out) CKM(cudaMemcpyAsync(row_valid_out, t->d_row_valid, static_cast<size_t>(B) * 4, cudaMemcpyDeviceToHost, t->stream));
-    }
-    cudaError_t e = cudaStreamSynchronize(t->stream);
-    if (e != cudaSuccess) return t->fail(DTX_ERR_CUDA, "eval failed on device: %s", cudaGetErrorString(e));
-    if (loss_out) *loss_out = h;
-    return DTX_OK;
-  }
-  SubPlan plan;
-  if (!t->full) plan_groups(PlanDims{t->mc.hidden, t->mc.ffn, t->W, t->dq, t->n_sms, B}, seq_lens, labels, t->cur_S, &plan);
-  if (plan.n > 1) {
-    // ragged batch as length groups (forward only): the per-row statistics come back in group order and are put back in
-    // the caller's row order; the batch loss accumulates over the groups with the whole batch's labelled-token count
-    const int S_src = t->cur_S;
-    CKM(cudaMemcpyAsync(t->d_ids_full, ids, static_cast<size_t>(t->cur_M) * 4, cudaMemcpyHostToDevice, t->stream));
-    CKM(cudaMemcpyAsync(t->d_labels_full, labels, static_cast<size_t>(t->cur_M) * 4, cudaMemcpyHostToDevice, t->stream));
-    CKM(cudaMemcpyAsync(t->d_lens_full, seq_lens, static_cast<size_t>(B) * 4, cudaMemcpyHostToDevice, t->stream));
-    t->h_row_sum.assign(static_cast<size_t>(B), 0.f);
-    t->h_row_valid.assign(static_cast<size_t>(B), 0);
-    for (int g = 0; g < plan.n && rc == DTX_OK; ++g) {
-      RowList rl;
-      rl.n = plan.start[g + 1] - plan.start[g];
-      for (int k = 0; k < rl.n; ++k) rl.rows[k] = plan.order[plan.start[g] + k];
-      cudaError_t ge = gather_rows(t->d_ids_full, t->d_labels_full, t->d_lens_full, S_src, rl, plan.S[g], t->d_ids, t->d_labels,
-                                   t->d_seq_lens, t->stream);
-      if (ge != cudaSuccess) rc = t->fail(DTX_ERR_CUDA, "gather_rows: %s", cudaGetErrorString(ge));
-      if (rc) break;
-      t->launches += 1;
-      t->cur_B = rl.n;
-      t->cur_S = plan.S[g];
-      t->cur_M = rl.n * plan.S[g];
-      t->use_seq_lens = true;
-      t->sub_accum = g > 0;
-      t->sub_ndiv = plan.n_div;
-      rc = fwd_bwd(t, false);
-      if (rc == DTX_OK && (row_sum_out || row_valid_out)) {
-        cudaError_t e2 = row_loss_stats(t->row_loss, t->d_shift, rl.n, t->cur_S, t->d_row_sum, t->d_row_valid, t->stream);
-        if (e2 == cudaSuccess) e2 = cudaMemcpyAsync(t->h_row_sum.data() + plan.start[g], t->d_row_sum, static_cast<size_t>(rl.n) * 4, cudaMemcpyDeviceToHost, t->stream);
-        if (e2 == cudaSuccess) e2 = cudaMemcpyAsync(t->h_row_valid.data() + plan.start[g], t->d_row_valid, static_cast<size_t>(rl.n) * 4, cudaMemcpyDeviceToHost, t->stream);
-        // d_row_sum / d_row_valid are reused by the next group: the copies above are stream-ordered in front of its kernels
-        if (e2 != cudaSuccess) rc = t->fail(DTX_ERR_CUDA, "eval row statistics: %s", cudaGetErrorString(e2));
-        t->launches += 1;
-      }
-    }
-    t->sub_accum = false;
-    t->sub_ndiv = 0;
-    if (rc) return rc;
-    CKM(cudaMemcpyAsync(&h, t->d_loss, 4, cudaMemcpyDeviceToHost, t->stream));
-    cudaError_t e = cudaStreamSynchronize(t->stream);
-    if (e != cudaSuccess) return t->fail(DTX_ERR_CUDA, "eval failed on device: %s", cudaGetErrorString(e));
-    for (int k = 0; k < B; ++k) {
-      if (row_sum_out) row_sum_out[plan.order[k]] = t->h_row_sum[static_cast<size_t>(k)];
-      if (row_valid_out) row_valid_out[plan.order[k]] = t->h_row_valid[static_cast<size_t>(k)];
-    }
-    if (loss_out) *loss_out = h;
-    return DTX_OK;
-  }
-  CKM(cudaMemcpyAsync(t->d_ids, ids, static_cast<size_t>(t->cur_M) * 4, cudaMemcpyHostToDevice, t->stream));
-  CKM(cudaMemcpyAsync(t->d_labels, labels, static_cast<size_t>(t->cur_M) * 4, cudaMemcpyHostToDevice, t->stream));
-  if (seq_lens) CKM(cudaMemcpyAsync(t->d_seq_lens, seq_lens, static_cast<size_t>(B) * 4, cudaMemcpyHostToDevice, t->stream));
-  rc = fwd_bwd(t, false);
+  RowStats rows{row_sum_out, row_valid_out};
+  const bool want_rows = row_sum_out || row_valid_out;
+  rc = run_batch(t, BatchInput{ids, labels, seq_lens, false, t->cur_S}, false, want_rows ? &rows : nullptr);
   if (rc) return rc;
+  float h = 0.f;
   CKM(cudaMemcpyAsync(&h, t->d_loss, 4, cudaMemcpyDeviceToHost, t->stream));
-  if (row_sum_out || row_valid_out) {
-    CK(row_loss_stats(t->row_loss, t->d_shift, B, t->cur_S, t->d_row_sum, t->d_row_valid, t->stream), 1);
-    if (row_sum_out) CKM(cudaMemcpyAsync(row_sum_out, t->d_row_sum, static_cast<size_t>(B) * 4, cudaMemcpyDeviceToHost, t->stream));
-    if (row_valid_out) CKM(cudaMemcpyAsync(row_valid_out, t->d_row_valid, static_cast<size_t>(B) * 4, cudaMemcpyDeviceToHost, t->stream));
-  }
   cudaError_t e = cudaStreamSynchronize(t->stream);
   if (e != cudaSuccess) return t->fail(DTX_ERR_CUDA, "eval failed on device: %s", cudaGetErrorString(e));
+  for (int k = 0; want_rows && k < t->tc.micro_batch; ++k) {
+    if (row_sum_out) row_sum_out[rows.order[k]] = t->h_row_sum[static_cast<size_t>(k)];
+    if (row_valid_out) row_valid_out[rows.order[k]] = t->h_row_valid[static_cast<size_t>(k)];
+  }
   if (loss_out) *loss_out = h;
   return DTX_OK;
 }

@@ -178,7 +178,9 @@ DTX_API int64_t dtx_base_weight_bytes(const dtx_trainer* t);
 DTX_API int32_t dtx_step(dtx_trainer* t, const int32_t* input_ids, const int32_t* labels, const int32_t* seq_lens,
                  int32_t seq_len_batch, int32_t flags, float* loss_out, float* grad_norm_out, float* lr_out,
                  int32_t* stepped_out);
-/* Same with the batch already resident on this trainer's device (int32 device pointers; d_seq_lens may be NULL). */
+/* Same with the batch already resident on this trainer's device (int32 device pointers; d_seq_lens may be NULL).  It makes the
+ * same layout decision as dtx_step (packed, length groups or one pass); to plan it, the row lengths - and, when length groups
+ * are planned, the labels - are read back to the host. */
 DTX_API int32_t dtx_step_device(dtx_trainer* t, const void* d_input_ids, const void* d_labels, const void* d_seq_lens,
                         int32_t seq_len_batch, int32_t flags, float* loss_out, float* grad_norm_out, float* lr_out,
                         int32_t* stepped_out);
@@ -244,7 +246,9 @@ DTX_API double dtx_lr_lambda(int32_t sched, int32_t step, int32_t warmup_steps, 
  * softmax's exponentials is computed on the FMA pipe (cubic polynomial) instead of MUFU.EX2 (default 0 = none: not measured on H100).
  * "attn_dq_exp_fma_every" = N in {0, 3, 4}: the same for the dQ kernel's exp / dS phase (default 0).
  * "varlen_split" = 1 (default): a LoRA micro-batch that comes with row lengths is run as length groups (rows sorted by length,
- * partition chosen by a cost model; same token-mean loss and gradients up to summation order); 0: one pass at the batch's length.
+ * partition chosen by a cost model; same token-mean loss and gradients up to summation order); 0: one pass at the batch's length;
+ * 2: never packed, and the groups are cut wherever the 128-rounded row lengths differ, without the cost model (parity tests at
+ * shapes too small for it to split).  Other values return DTX_ERR_INVALID.
  * "varlen_pack" = 1 (default): such a micro-batch (LoRA or full-parameter) is instead run PACKED - sequences back to back at their
  * 128-rounded lengths, one pass - whenever the fused RoPE epilogue applies (q|k|v width a multiple of 256); 0: length groups.
  * "varlen_group_cost" = N: fixed cost the partition's cost model charges per group, in thousandths of one wave of every GEMM of a layer.

@@ -68,3 +68,9 @@ def test_option_switches_are_known_and_unknown_names_rejected(lib):
         L.set_option(name, value)  # restores the default: raises DtxError on an unknown name
     with pytest.raises(L.DtxError):
         L.set_option("no_such_option", 1)
+    for value in (0, 1, 2):
+        L.set_option("varlen_split", value)
+    for value in (3, -1):
+        with pytest.raises(L.DtxError):
+            L.set_option("varlen_split", value)
+    L.set_option("varlen_split", 1)

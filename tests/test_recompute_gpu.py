@@ -2,7 +2,8 @@
 pass with the very same launches, so every result must be BITWISE the one of the "keep" layout - losses, grad norms, learning
 rates, trained adapters / weights, their gradients and the evaluation row statistics - across the features the forward pass
 has (GQA, LoRA dropout, accumulation, NF4 with side-stream prefetch, packed and length-grouped ragged batches, sliding window,
-full-parameter SFT)."""
+full-parameter SFT).  The same harness checks that the host-buffer and the device-pointer step entries lay a batch out the same
+way and compute the same bits with the same launches."""
 import dataclasses
 
 import numpy as np
@@ -42,8 +43,10 @@ def _batches(vocab, B, S, n, lens_list=None):
     return out
 
 
-def _train(mc, tc, layout, batches, quant=False, eval_batches=(), options=None):
-    """Train on `batches` from seeded weights with activation layout `layout`; everything the run returns, as bytes."""
+def _train(mc, tc, layout, batches, quant=False, eval_batches=(), options=None, entry="host", launches=False):
+    """Train on `batches` from seeded weights with activation layout `layout`; everything the run returns, as bytes.
+    entry "host": numpy batches through dtx_step; "device": CUDA tensors through dtx_step_device.  launches: also record the
+    kernel launches of every step."""
     L = _lib()
     options = options or {}
     defaults = {"varlen_pack": 1, "varlen_split": 1}
@@ -57,13 +60,23 @@ def _train(mc, tc, layout, batches, quant=False, eval_batches=(), options=None):
             tr.quantize_base("int4")
         if not tc.full_finetune:
             tr.init_lora(4321)
-        trace, groups, evals = [], [], []
+        trace, groups, evals, counts = [], [], [], []
         for ids, labels, lens in batches:
-            trace.append(tr.step(ids, labels, lens))
+            before = tr.launch_count
+            if entry == "host":
+                trace.append(tr.step(ids, labels, lens))
+            else:
+                import torch
+                d = [torch.from_numpy(a).cuda() for a in (ids, labels) + ((lens,) if lens is not None else ())]
+                torch.cuda.synchronize()  # the trainer's stream does not order itself after torch's
+                trace.append(tr.step_ptr(d[0].data_ptr(), d[1].data_ptr(), True, d[2].data_ptr() if lens is not None else 0,
+                                         ids.shape[1]))
+            counts.append(tr.launch_count - before)
             groups.append(tr.last_step_groups)
         for ids, labels, lens in eval_batches:
             sums, cnts = tr.eval_rows(ids, labels, lens)
             evals.append((sums.tobytes(), cnts.tobytes(), tr.eval_loss(ids, labels, lens)))
+            assert tr.last_step_groups == groups[-1], "evaluation changed last_step_groups"
         if tc.full_finetune:
             state = {k: v.tobytes() for k, v in tr.export_weights().items()}
             grads = {k: v.tobytes() for k, v in tr.export_weights(grads=True).items()}
@@ -74,7 +87,10 @@ def _train(mc, tc, layout, batches, quant=False, eval_batches=(), options=None):
         tr.close()
         for k in options:
             L.set_option(k, defaults[k])
-    return {"trace": trace, "groups": groups, "eval": evals, "state": state, "grads": grads}
+    out = {"trace": trace, "groups": groups, "eval": evals, "state": state, "grads": grads}
+    if launches:
+        out["launches"] = counts
+    return out
 
 
 def _tiny(S=256, B=2, layers=3, heads=2, kv_heads=None, dropout=0.0, targets=("q_proj", "v_proj"), **mkw):
@@ -127,6 +143,16 @@ def _case(name):
         if name == "full_accum":
             tc.grad_accum = 2
         return mc, tc, _batches(2048, 2, 256, 8 if name == "full_accum" else 4), {}
+    if name == "full_packed":
+        mc, tc = _tiny(S=512, B=4)
+        tc.full_finetune = True
+        tc.lr = 1e-4
+        b = _batches(2048, 4, 512, 4, PACKED_LENS)
+        return mc, tc, b, {"eval_batches": b[:2]}
+    if name == "padded_lens":  # one pass at the padded shape that still carries the row lengths
+        mc, tc = _tiny(S=512, B=4)
+        b = _batches(2048, 4, 512, 4, PACKED_LENS)
+        return mc, tc, b, {"eval_batches": b[:2], "options": {"varlen_pack": 0, "varlen_split": 0}}
     if name == "layer4_7b_width":
         L = _lib()
         mc = L.ModelConfig(vocab=32000, hidden=4096, n_layers=4, n_heads=32, ffn=11008)
@@ -155,6 +181,30 @@ def test_layer_recompute_is_bitwise_keep_all(name):
     diff = [k for k in keep["state"] if keep["state"][k] != layer["state"][k]]
     assert not diff, f"trained tensors differ: {diff[:5]}"
     diff = [k for k in keep["grads"] if keep["grads"][k] != layer["grads"][k]]
+    assert not diff, f"gradients differ: {diff[:5]}"
+
+
+@pytest.mark.parametrize("name", ["tiny_qv", "dropout", "grad_accum", "packed", "length_groups", "qlora_groups", "full_accum",
+                                  "full_packed", "padded_lens"])
+def test_host_and_device_entries_are_bitwise_equal(name):
+    """dtx_step and dtx_step_device lay a batch out the same way: same groups, same launches, bitwise the same results."""
+    mc, tc, batches, kw = _case(name)
+    host = _train(mc, tc, "keep", batches, entry="host", launches=True, **kw)
+    dev = _train(mc, tc, "keep", batches, entry="device", launches=True, **kw)
+    assert host["groups"] == dev["groups"], (host["groups"], dev["groups"])
+    if name in ("packed", "full_packed"):
+        assert 0 in host["groups"], host["groups"]
+    if name in ("length_groups", "qlora_groups"):
+        assert max(host["groups"]) >= 2, host["groups"]
+    if name == "padded_lens":
+        assert set(host["groups"]) == {1}, host["groups"]
+    assert host["launches"] == dev["launches"], (host["launches"], dev["launches"])
+    assert host["trace"] == dev["trace"], list(zip(host["trace"], dev["trace"]))
+    assert host["eval"] == dev["eval"]
+    assert host["state"].keys() == dev["state"].keys()
+    diff = [k for k in host["state"] if host["state"][k] != dev["state"][k]]
+    assert not diff, f"trained tensors differ: {diff[:5]}"
+    diff = [k for k in host["grads"] if host["grads"][k] != dev["grads"][k]]
     assert not diff, f"gradients differ: {diff[:5]}"
 
 
