@@ -117,6 +117,21 @@ int32_t dtx_post_norm_add(const void* y, const void* w, const void* res, void* o
                           static_cast<float*>(rstd), M, d, eps, S(stream)));
 }
 
+int32_t dtx_qk_norm_full_rope_fwd(void* qkv, int64_t ld, int32_t M, int32_t q_cols, int32_t n_cols, const void* wq, const void* wk,
+                                  float eps, const void* cs_table, int32_t rope_S, const void* rope_pos, void* pre, int64_t ld_pre,
+                                  void* stream) {
+  return rc(qk_norm_full_rope_fwd(static_cast<bf16*>(qkv), ld, M, q_cols, n_cols, static_cast<const bf16*>(wq), static_cast<const bf16*>(wk),
+                                  eps, static_cast<const float2*>(cs_table), rope_S, static_cast<const int32_t*>(rope_pos),
+                                  static_cast<bf16*>(pre), ld_pre, S(stream)));
+}
+
+int32_t dtx_qk_norm_full_bwd(void* dy, int64_t ld, const void* x, int64_t ldx, int32_t M, int32_t q_cols, int32_t n_cols, const void* wq,
+                             const void* wk, float eps, void* dw, void* scratch, int32_t accumulate, void* stream) {
+  return rc(qk_norm_full_bwd(static_cast<bf16*>(dy), ld, static_cast<const bf16*>(x), ldx, M, q_cols, n_cols, static_cast<const bf16*>(wq),
+                             static_cast<const bf16*>(wk), eps, static_cast<bf16*>(dw), static_cast<float*>(scratch), accumulate,
+                             S(stream)));
+}
+
 int32_t dtx_set_option(const char* name, int32_t value) {
   if (!name) return DTX_ERR_INVALID;
   if (strcmp(name, "gemm_pair_kernel") == 0) {

@@ -949,6 +949,176 @@ __global__ void __launch_bounds__(256) qk_norm_dw_kernel(const float* __restrict
   if (accumulate) v += __bfloat162float(dw[c]);
   dw[c] = __float2bfloat16_rn(v);
 }
+// ------------------------------------------------------------------------------------------
+// OLMo-2 q/k RMSNorm over the full width of a row: one norm over the q columns [0, q_cols) with weight wq [q_cols], another
+// over the k columns [q_cols, n_cols) with weight wk [n_cols - q_cols].  The sums span all heads of a row, so they cannot
+// run in the q|k|v GEMM's epilogue (one tile holds 256 columns): one HBM-bound pass after the plain GEMM instead.
+// ------------------------------------------------------------------------------------------
+constexpr int QKF_FWD_THREADS = 128, QKF_BWD_THREADS = 256;
+// Forward, in place, one block per row.  A unit is 8 columns of the low half of a head and the matching 8 of its high half
+// (the rotary pairs i, i + 64), so the row stays in registers between the two sums and the scale + rotary:
+//   pre = x;  x = rotary((x * rsqrt(mean(x^2) + eps)) * w)   in fp32, rounded once (as EPI_ROPE rounds the rotated accumulator).
+// Position: pos[row] (packed batch), else row % S; cs = [S][64] float2 (cos, sin).
+template <int NCH>
+__global__ void __launch_bounds__(QKF_FWD_THREADS) qk_norm_full_rope_fwd_kernel(
+    bf16* __restrict__ qkv, long long ld, int q_cols, int n_cols, const bf16* __restrict__ wq, const bf16* __restrict__ wk, float eps,
+    const float2* __restrict__ cs, int S, const int32_t* __restrict__ pos, bf16* __restrict__ pre, long long ld_pre) {
+  __shared__ float sh[2][4];
+  const int row = blockIdx.x, nu = n_cols >> 4;
+  bf16* xr = qkv + row * ld;
+  bf16* pr = pre + row * ld_pre;
+  uint4 lo[NCH], hi[NCH];
+#pragma unroll
+  for (int i = 0; i < NCH; ++i) {
+    const int u = i * QKF_FWD_THREADS + threadIdx.x;
+    if (u < nu) {
+      const int c = (u >> 3) * 128 + (u & 7) * 8;
+      lo[i] = *reinterpret_cast<const uint4*>(xr + c);
+      hi[i] = *reinterpret_cast<const uint4*>(xr + c + 64);
+    }
+  }
+  float sq = 0.f, sk = 0.f;
+#pragma unroll
+  for (int i = 0; i < NCH; ++i) {
+    const int u = i * QKF_FWD_THREADS + threadIdx.x;
+    if (u < nu) {
+      const int c = (u >> 3) * 128 + (u & 7) * 8;
+      *reinterpret_cast<uint4*>(pr + c) = lo[i];
+      *reinterpret_cast<uint4*>(pr + c + 64) = hi[i];
+      float a[8], b[8], s = 0.f;
+      bf16x8_to_f32(lo[i], a);
+      bf16x8_to_f32(hi[i], b);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) s += a[j] * a[j] + b[j] * b[j];
+      if (c < q_cols) sq += s;
+      else sk += s;
+    }
+  }
+  sq = block_sum_128(sq, sh[0]);
+  sk = block_sum_128(sk, sh[1]);
+  const float rq = rsqrtf(sq / static_cast<float>(q_cols) + eps), rk = rsqrtf(sk / static_cast<float>(n_cols - q_cols) + eps);
+  const int p = pos ? pos[row] : row % S;
+#pragma unroll
+  for (int i = 0; i < NCH; ++i) {
+    const int u = i * QKF_FWD_THREADS + threadIdx.x;
+    if (u < nu) {
+      const int c = (u >> 3) * 128 + (u & 7) * 8;
+      const bool is_q = c < q_cols;
+      const float r = is_q ? rq : rk;
+      const bf16* w = is_q ? wq + c : wk + (c - q_cols);
+      float a[8], b[8], wa[8], wb[8];
+      bf16x8_to_f32(lo[i], a);
+      bf16x8_to_f32(hi[i], b);
+      bf16x8_to_f32(__ldg(reinterpret_cast<const uint4*>(w)), wa);
+      bf16x8_to_f32(__ldg(reinterpret_cast<const uint4*>(w + 64)), wb);
+      const float2* t = cs + static_cast<size_t>(p) * 64 + (u & 7) * 8;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float2 v = __ldg(t + j);
+        const float x0 = a[j] * r * wa[j], x1 = b[j] * r * wb[j];
+        a[j] = x0 * v.x - x1 * v.y;
+        b[j] = x1 * v.x + x0 * v.y;
+      }
+      *reinterpret_cast<uint4*>(xr + c) = f32_to_bf16x8(a);
+      *reinterpret_cast<uint4*>(xr + c + 64) = f32_to_bf16x8(b);
+    }
+  }
+}
+// four block-wide sums of a 256-thread block in a fixed order; sh is free again once every thread has returned
+__device__ __forceinline__ float4 block_sum4_256(float4 v, float (*sh)[8]) {
+  v.x = warp_sum(v.x); v.y = warp_sum(v.y); v.z = warp_sum(v.z); v.w = warp_sum(v.w);
+  const int w = threadIdx.x >> 5;
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) { sh[0][w] = v.x; sh[1][w] = v.y; sh[2][w] = v.z; sh[3][w] = v.w; }
+  __syncthreads();
+  float r[4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) r[k] = ((sh[k][0] + sh[k][1]) + (sh[k][2] + sh[k][3])) + ((sh[k][4] + sh[k][5]) + (sh[k][6] + sh[k][7]));
+  return make_float4(r[0], r[1], r[2], r[3]);
+}
+// Backward, in place on dy (after the inverse rotary), rows blockIdx.x, blockIdx.x + gridDim.x, ...; 8 consecutive columns per
+// unit.  rstd is recomputed from the saved pre-norm x:  dx = rstd * (w*dy) - x * rstd^3 * mean(w*dy*x)  per span.
+// part (optional, [gridDim.x][n_cols] fp32): block b's sums of dy * x * rstd over its rows, each column in one thread's
+// registers in row order - the first stage of the weight gradient, rmsnorm_dw_stage2 is the second.
+template <int NCH>
+__global__ void __launch_bounds__(QKF_BWD_THREADS) qk_norm_full_bwd_kernel(bf16* __restrict__ dy, long long ld, const bf16* __restrict__ xs,
+                                                                           long long ldx, int M, int q_cols, int n_cols,
+                                                                           const bf16* __restrict__ wq, const bf16* __restrict__ wk,
+                                                                           float eps, float* __restrict__ part) {
+  __shared__ float sh[4][8];
+  const int nu = n_cols >> 3;
+  float acc[NCH][8];
+#pragma unroll
+  for (int i = 0; i < NCH; ++i)
+#pragma unroll
+    for (int j = 0; j < 8; ++j) acc[i][j] = 0.f;
+  for (int row = blockIdx.x; row < M; row += gridDim.x) {
+    bf16* gr = dy + row * ld;
+    const bf16* xr = xs + row * ldx;
+    uint4 bx[NCH], bg[NCH];
+#pragma unroll
+    for (int i = 0; i < NCH; ++i) {
+      const int u = i * QKF_BWD_THREADS + threadIdx.x;
+      if (u < nu) {
+        bx[i] = ldg_stream(reinterpret_cast<const uint4*>(xr) + u);
+        bg[i] = *(reinterpret_cast<const uint4*>(gr) + u);
+      }
+    }
+    float4 s = make_float4(0.f, 0.f, 0.f, 0.f);  // sum x^2 (q, k), sum w*dy*x (q, k)
+#pragma unroll
+    for (int i = 0; i < NCH; ++i) {
+      const int u = i * QKF_BWD_THREADS + threadIdx.x;
+      if (u < nu) {
+        const int c = u * 8;
+        const bool is_q = c < q_cols;
+        float fx[8], fg[8], fw[8], ss = 0.f, dot = 0.f;
+        bf16x8_to_f32(bx[i], fx);
+        bf16x8_to_f32(bg[i], fg);
+        bf16x8_to_f32(__ldg(reinterpret_cast<const uint4*>(is_q ? wq + c : wk + (c - q_cols))), fw);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          ss += fx[j] * fx[j];
+          dot += fg[j] * fw[j] * fx[j];
+        }
+        if (is_q) { s.x += ss; s.z += dot; }
+        else { s.y += ss; s.w += dot; }
+      }
+    }
+    s = block_sum4_256(s, sh);
+    const float nq = static_cast<float>(q_cols), nk = static_cast<float>(n_cols - q_cols);
+    const float rq = rsqrtf(s.x / nq + eps), rk = rsqrtf(s.y / nk + eps);
+    const float cq = s.z * rq * rq * rq / nq, ck = s.w * rk * rk * rk / nk;
+#pragma unroll
+    for (int i = 0; i < NCH; ++i) {
+      const int u = i * QKF_BWD_THREADS + threadIdx.x;
+      if (u < nu) {
+        const int c = u * 8;
+        const bool is_q = c < q_cols;
+        const float r = is_q ? rq : rk, cc = is_q ? cq : ck;
+        float fx[8], fg[8], fw[8], o[8];
+        bf16x8_to_f32(bx[i], fx);
+        bf16x8_to_f32(bg[i], fg);
+        bf16x8_to_f32(__ldg(reinterpret_cast<const uint4*>(is_q ? wq + c : wk + (c - q_cols))), fw);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          if (part) acc[i][j] += fg[j] * fx[j] * r;
+          o[j] = fg[j] * fw[j] * r - fx[j] * cc;
+        }
+        *(reinterpret_cast<uint4*>(gr) + u) = f32_to_bf16x8(o);
+      }
+    }
+  }
+  if (!part) return;
+#pragma unroll
+  for (int i = 0; i < NCH; ++i) {
+    const int u = i * QKF_BWD_THREADS + threadIdx.x;
+    if (u < nu) {
+      float4* dst = reinterpret_cast<float4*>(part + static_cast<size_t>(blockIdx.x) * n_cols + u * 8);
+      dst[0] = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
+      dst[1] = make_float4(acc[i][4], acc[i][5], acc[i][6], acc[i][7]);
+    }
+  }
+}
 __global__ void embedding_bwd_kernel(const int32_t* __restrict__ ids, const bf16* __restrict__ dx, float* __restrict__ dE, int d, int vocab) {
   const int m = blockIdx.x;
   const int id = ids[m];
@@ -1257,6 +1427,38 @@ cudaError_t qk_norm_bwd(bf16* dy, int64_t ld, const bf16* x, int64_t ldx, int M,
   const int grid = dw ? nblk : qk_norm_grid(M, n_cols);
   qk_norm_bwd_kernel<<<grid, 256, 0, s>>>(dy, ld, x, ldx, M, q_cols, n_cols, wq, wk, eps, dw ? scratch : nullptr);
   if (dw) qk_norm_dw_kernel<<<256 / 32, 256, 0, s>>>(scratch, nblk, dw, accumulate);
+  return cudaGetLastError();
+}
+namespace {
+bool aligned16(const void* p) { return !(reinterpret_cast<uintptr_t>(p) & 15); }
+bool qk_norm_full_args_ok(const void* x, int64_t ld, const void* y, int64_t ldy, int M, int q_cols, int n_cols, const bf16* wq,
+                          const bf16* wk, float eps) {
+  return x && y && wq && wk && M > 0 && q_cols > 0 && !(q_cols & 127) && n_cols > q_cols && !(n_cols & 127) && n_cols <= QKF_MAX_COLS &&
+         ld >= n_cols && ldy >= n_cols && !(ld & 7) && !(ldy & 7) && aligned16(x) && aligned16(y) && aligned16(wq) && aligned16(wk) &&
+         eps >= 0.f;
+}
+}  // namespace
+cudaError_t qk_norm_full_rope_fwd(bf16* qkv, int64_t ld, int M, int q_cols, int n_cols, const bf16* wq, const bf16* wk, float eps,
+                                  const float2* cs, int S, const int32_t* pos, bf16* pre, int64_t ld_pre, cudaStream_t s) {
+  if (!qk_norm_full_args_ok(qkv, ld, pre, ld_pre, M, q_cols, n_cols, wq, wk, eps) || !cs || S <= 0) return cudaErrorInvalidValue;
+  const int nch = (n_cols / 16 + QKF_FWD_THREADS - 1) / QKF_FWD_THREADS;
+  if (nch <= 1) qk_norm_full_rope_fwd_kernel<1><<<M, QKF_FWD_THREADS, 0, s>>>(qkv, ld, q_cols, n_cols, wq, wk, eps, cs, S, pos, pre, ld_pre);
+  else if (nch <= 2) qk_norm_full_rope_fwd_kernel<2><<<M, QKF_FWD_THREADS, 0, s>>>(qkv, ld, q_cols, n_cols, wq, wk, eps, cs, S, pos, pre, ld_pre);
+  else if (nch <= 4) qk_norm_full_rope_fwd_kernel<4><<<M, QKF_FWD_THREADS, 0, s>>>(qkv, ld, q_cols, n_cols, wq, wk, eps, cs, S, pos, pre, ld_pre);
+  else qk_norm_full_rope_fwd_kernel<8><<<M, QKF_FWD_THREADS, 0, s>>>(qkv, ld, q_cols, n_cols, wq, wk, eps, cs, S, pos, pre, ld_pre);
+  return cudaGetLastError();
+}
+cudaError_t qk_norm_full_bwd(bf16* dy, int64_t ld, const bf16* x, int64_t ldx, int M, int q_cols, int n_cols, const bf16* wq, const bf16* wk,
+                             float eps, bf16* dw, float* scratch, int accumulate, cudaStream_t s) {
+  if (!qk_norm_full_args_ok(dy, ld, x, ldx, M, q_cols, n_cols, wq, wk, eps) || (dw && (!scratch || !aligned16(scratch)))) return cudaErrorInvalidValue;
+  const int nch = (n_cols / 8 + QKF_BWD_THREADS - 1) / QKF_BWD_THREADS;
+  const int grid = dw ? NDW_ROWBLOCKS : M;
+  float* part = dw ? scratch : nullptr;
+  if (nch <= 1) qk_norm_full_bwd_kernel<1><<<grid, QKF_BWD_THREADS, 0, s>>>(dy, ld, x, ldx, M, q_cols, n_cols, wq, wk, eps, part);
+  else if (nch <= 2) qk_norm_full_bwd_kernel<2><<<grid, QKF_BWD_THREADS, 0, s>>>(dy, ld, x, ldx, M, q_cols, n_cols, wq, wk, eps, part);
+  else if (nch <= 4) qk_norm_full_bwd_kernel<4><<<grid, QKF_BWD_THREADS, 0, s>>>(dy, ld, x, ldx, M, q_cols, n_cols, wq, wk, eps, part);
+  else qk_norm_full_bwd_kernel<8><<<grid, QKF_BWD_THREADS, 0, s>>>(dy, ld, x, ldx, M, q_cols, n_cols, wq, wk, eps, part);
+  if (dw) rmsnorm_dw_stage2<<<(n_cols + 255) / 256, 256, 0, s>>>(scratch, n_cols, dw, accumulate);
   return cudaGetLastError();
 }
 cudaError_t embedding_bwd(const int32_t* ids, const bf16* dx, float* dE32, int M, int d, int vocab, cudaStream_t s) {

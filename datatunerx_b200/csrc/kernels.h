@@ -211,6 +211,18 @@ cudaError_t qk_norm_fwd(bf16* qkv, int64_t ld, int M, int q_cols, int n_cols, co
 constexpr int QKN_MAX_BLOCKS = 1024;
 cudaError_t qk_norm_bwd(bf16* dy, int64_t ld, const bf16* x, int64_t ldx, int M, int q_cols, int n_cols, const bf16* wq, const bf16* wk,
                         float eps, bf16* dw, float* scratch, int nblk, int accumulate, cudaStream_t s);
+// OLMo-2 q/k RMSNorm over the full width of a row: one norm over columns [0, q_cols) with weight wq [q_cols], one over
+// [q_cols, n_cols) with weight wk [n_cols - q_cols] (both spans multiples of 128, n_cols <= QKF_MAX_COLS, 16-byte aligned rows).
+// Forward, in place, then the half-split rotary (pairs i / i + 64 of every head, cs = [S][64] float2, position pos[m] or m % S):
+//   pre[m, c] = x,  x = rotary((x * rsqrt(mean(x^2) + eps)) * w)   in fp32, one rounding.
+constexpr int QKF_MAX_COLS = 16384;
+cudaError_t qk_norm_full_rope_fwd(bf16* qkv, int64_t ld, int M, int q_cols, int n_cols, const bf16* wq, const bf16* wk, float eps,
+                                  const float2* cs, int S, const int32_t* pos, bf16* pre, int64_t ld_pre, cudaStream_t s);
+// Backward, in place on dy (after the inverse rotary): dx = rstd * (w*dy - xh * mean(w*dy*xh)) per span, xh = x * rstd recomputed
+// from the saved pre-norm x.  dw (optional, bf16 [n_cols] = [d q_norm | d k_norm]) (+)= sum_m dy * xh: 64 blocks write fp32
+// per-block sums to scratch (>= 64 * n_cols floats), rmsnorm_dw's second stage adds them in a fixed order (no atomics).
+cudaError_t qk_norm_full_bwd(bf16* dy, int64_t ld, const bf16* x, int64_t ldx, int M, int q_cols, int n_cols, const bf16* wq, const bf16* wk,
+                             float eps, bf16* dw, float* scratch, int accumulate, cudaStream_t s);
 // dst[i] = (accumulate ? dst[i] : 0) + src[i]   fp32 -> bf16
 cudaError_t add_f32_into_bf16(const float* src, bf16* dst, int64_t n, int accumulate, cudaStream_t s);
 // *out (+)= sum g[i]^2 over a bf16 buffer (two-stage, fixed order; first = 1 overwrites)

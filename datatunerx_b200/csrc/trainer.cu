@@ -150,13 +150,14 @@ struct Layer {
   bf16 *wqkv = nullptr, *wo = nullptr, *wgu = nullptr, *wdown = nullptr, *norm1 = nullptr, *norm2 = nullptr;
   bf16* bias = nullptr;  // dtx_model_ext.qkv_bias: [W] q|k|v biases in the row order of wqkv (bf16 also under NF4), else null
   bf16* qkn = nullptr;   // dtx_model_ext.qk_norm: [2 * 128] q_norm | k_norm weights (bf16 also under NF4), else null
-  bf16* qk_pre = nullptr;  // qk_norm, saved: [M, dq + dkv] q|k projection output before the norm (bf16)
+  bf16* qkf = nullptr;   // dtx_model_ext.qk_norm_full: [dq + dkv] q_norm | k_norm weights (bf16 also under NF4), else null
+  bf16* qk_pre = nullptr;  // qk_norm / qk_norm_full, saved: [M, dq + dkv] q|k projection output before the norm (bf16)
   bf16* pn = nullptr;  // dtx_model_ext.post_norms: [2 * d] post_self_attn_layernorm | post_mlp_layernorm (bf16 also under NF4)
   // post_norms, saved: the o- and down-projection outputs before their norms [M, d] and the norms' rstd [M]
   bf16 *o_pre = nullptr, *down_pre = nullptr;
   float *rstd_pn1 = nullptr, *rstd_pn2 = nullptr;
   bf16 *a_cat = nullptr, *b_ext = nullptr;                                               // shadows
-  bf16 *h1 = nullptr, *t = nullptr, *qkv = nullptr, *attn = nullptr, *x_mid = nullptr, *gu = nullptr;  // saved
+  bf16 *h1 = nullptr, *t = nullptr, *qkv = nullptr, *attn = nullptr, *x_mid = nullptr, *gu = nullptr;  // saved (no_pre_norms: no h1)
   bf16* hd = nullptr;  // LoRA dropout only: [M, nt*d] dropped copies of h1, one per target (peft: one nn.Dropout per module)
   float *lse = nullptr, *rstd1 = nullptr, *rstd2 = nullptr;
   // --quantization int4: packed NF4 codes (two per byte) + one fp32 absmax per 64 elements; the bf16 pointers above are then
@@ -479,7 +480,8 @@ int create_buffers(dtx_trainer* t) {
     const size_t total = L * t->layer_elems + t->glob_elems, shard = total / t->world;
     ok = ok && t->alloc(&t->w_flat, total) && t->alloc(&t->g_flat, total);
     ok = ok && t->alloc(&t->master, shard) && t->alloc(&t->fm, shard) && t->alloc(&t->fv, shard);
-    ok = ok && t->alloc(&t->embed_g32, V * d) && t->alloc(&t->ndw_scratch, 64 * d);
+    // the norms' weight-gradient partials: 64 rows of the widest normalised span (qk_norm_full: the q|k columns)
+    ok = ok && t->alloc(&t->embed_g32, V * d) && t->alloc(&t->ndw_scratch, 64 * (t->ext.qk_norm_full ? std::max(d, QK) : d));
     if (!ok) return DTX_ERR_CUDA;
     CKM(t->zero(t->w_flat, total));
     CKM(t->zero(t->g_flat, total));
@@ -518,14 +520,15 @@ int create_buffers(dtx_trainer* t) {
       continue;
     }
     if (!full) ok = ok && t->alloc(&y.t, M * RP);
-    ok = ok && t->alloc(&y.h1, M * d) && t->alloc(&y.qkv, M * W) &&
-         t->alloc(&y.attn, M * dq) && t->alloc(&y.x_mid, M * d) && t->alloc(&y.gu, M * 2 * F);
-    if (t->ext.qk_norm) ok = ok && t->alloc(&y.qk_pre, M * QK);
+    const bool pre_norms = !t->ext.no_pre_norms;  // else the sublayers read xs[l] / x_mid: no h1, rstd1, rstd2
+    if (pre_norms) ok = ok && t->alloc(&y.h1, M * d);
+    ok = ok && t->alloc(&y.qkv, M * W) && t->alloc(&y.attn, M * dq) && t->alloc(&y.x_mid, M * d) && t->alloc(&y.gu, M * 2 * F);
+    if (t->ext.qk_norm || t->ext.qk_norm_full) ok = ok && t->alloc(&y.qk_pre, M * QK);
     if (t->ext.post_norms)
       ok = ok && t->alloc(&y.o_pre, M * d) && t->alloc(&y.down_pre, M * d) && t->alloc(&y.rstd_pn1, M) && t->alloc(&y.rstd_pn2, M);
     if (t->dropout) ok = ok && t->alloc(&y.hd, M * KA);
-    ok = ok && t->alloc(&y.lse, static_cast<size_t>(tc.micro_batch) * mc.n_heads * tc.seq_len) && t->alloc(&y.rstd1, M) &&
-         t->alloc(&y.rstd2, M);
+    ok = ok && t->alloc(&y.lse, static_cast<size_t>(tc.micro_batch) * mc.n_heads * tc.seq_len);
+    if (pre_norms) ok = ok && t->alloc(&y.rstd1, M) && t->alloc(&y.rstd2, M);
   }
   if (!ok) return DTX_ERR_CUDA;
   if (!full) {
@@ -736,11 +739,13 @@ int layer_fwd(dtx_trainer* t, int l, int phase, bool backward) {
   Layer& y = t->layers[l];
   const bf16* qk_wq = y.qkn;  // q_norm | k_norm (Qwen3), else null
   const bf16* qk_wk = y.qkn ? y.qkn + D : nullptr;
+  const bool pre_norms = !t->ext.no_pre_norms;  // else (OLMo-2) the sublayers read the residual stream itself
+  const bf16* h1 = pre_norms ? y.h1 : t->xs[l];
   wait_weights(t, l);
-  CK(rmsnorm_fwd(t->xs[l], y.norm1, y.h1, y.rstd1, M, d, mc.rms_eps, s), 1);
-  const bf16* lora_in = y.h1;
+  if (pre_norms) CK(rmsnorm_fwd(t->xs[l], y.norm1, y.h1, y.rstd1, M, d, mc.rms_eps, s), 1);
+  const bf16* lora_in = h1;
   if (drop) {  // peft: lora_A(lora_dropout(x)) with one nn.Dropout per wrapped module -> one dropped copy per target
-    CK(lora_dropout_fwd(y.h1, y.hd, M, d, t->nt, p_drop, dropout_key(t, l), s), 1);
+    CK(lora_dropout_fwd(h1, y.hd, M, d, t->nt, p_drop, dropout_key(t, l), s), 1);
     lora_in = y.hd;
   }
   if (lora) {  // LoRA down-projection of all targets at once: t = lora_in * A_cat^T   [M, RP]
@@ -752,11 +757,13 @@ int layer_fwd(dtx_trainer* t, int l, int phase, bool backward) {
   {  // qkv = h1 * Wqkv^T + t * B_ext^T : base projection and LoRA up-projection in one accumulator
     BASEW(W_QKV, wqkv);
     GemmArgs g;
-    g.A = y.h1; g.lda = d; g.B = wqkv; g.ldb = d;
+    g.A = h1; g.lda = d; g.B = wqkv; g.ldb = d;
     if (lora) { g.A2 = y.t; g.lda2 = RP; g.B2 = y.b_ext; g.ldb2 = RP; g.K2 = RP; }
     g.C = y.qkv; g.ldc = W; g.M = M; g.N = W; g.K = d; g.epilogue = EPI_BF16;
     g.bias = y.bias;  // q|k|v biases (Qwen2): added to the accumulator before the rounding / the rotary
-    if (fused) {  // rotary embedding of q and k applied to the fp32 accumulator in the epilogue
+    // rotary embedding of q and k applied to the fp32 accumulator in the epilogue; not with OLMo-2's full-width q/k norm, whose
+    // sums span more columns than a tile: its own pass below does norm + rotary
+    if (fused && !y.qkf) {
       g.epilogue = EPI_ROPE; g.rope_cs = t->rope_cs; g.rope_S = S; g.rope_cols = t->dq + t->dkv;
       g.rope_pos = t->packed ? t->d_pos : nullptr;  // packed batch: a row's position is its offset inside its own sequence
       if (qk_wq) {  // q/k norm (Qwen3) before the rotary; the pre-norm q|k is saved for the backward pass
@@ -767,9 +774,12 @@ int layer_fwd(dtx_trainer* t, int l, int phase, bool backward) {
     CK(gemm_bf16(g, s), 1);
   }
   if (!fused && t->packed) return t->fail(DTX_ERR_STATE, "packed batches need the fused RoPE epilogue");
-  if (!fused && qk_wq) CK(qk_norm_fwd(y.qkv, W, M, dq, QK, qk_wq, qk_wk, mc.rms_eps, y.qk_pre, QK, s), 1);
+  if (y.qkf)  // q|k = rotary(norm(q|k)) in place, the GEMM's bf16 q|k saved for the backward pass
+    CK(qk_norm_full_rope_fwd(y.qkv, W, M, dq, QK, y.qkf, y.qkf + dq, mc.rms_eps, t->rope_cs, S, t->packed ? t->d_pos : nullptr, y.qk_pre,
+                             QK, s), 1);
+  else if (!fused && qk_wq) CK(qk_norm_fwd(y.qkv, W, M, dq, QK, qk_wq, qk_wk, mc.rms_eps, y.qk_pre, QK, s), 1);
   if (!fused && t->rope_glm) CK(rope_glm_qk_inplace(y.qkv, t->rope_cs, B, S, H + Hkv, W, 0, s), 1);
-  else if (!fused) CK(rope_qk_inplace_table(y.qkv, t->rope_cs, B, S, H + Hkv, W, D, 0, s), 1);
+  else if (!fused && !y.qkf) CK(rope_qk_inplace_table(y.qkv, t->rope_cs, B, S, H + Hkv, W, D, 0, s), 1);
   {
     AttnArgs a;
     a.qkv = y.qkv; a.out = y.attn; a.lse = y.lse; a.B = B; a.S = S; a.H = H; a.Hkv = Hkv; a.scale = att_scale;
@@ -786,11 +796,11 @@ int layer_fwd(dtx_trainer* t, int l, int phase, bool backward) {
     CK(gemm_bf16(g, s), 1);
   }
   if (y.pn) CK(post_norm_add(y.o_pre, y.pn, t->xs[l], y.x_mid, y.rstd_pn1, M, d, mc.rms_eps, s), 1);
-  CK(rmsnorm_fwd(y.x_mid, y.norm2, t->h2, y.rstd2, M, d, mc.rms_eps, s), 1);
-  {  // [gate | up] = h2 * Wgu^T
+  if (pre_norms) CK(rmsnorm_fwd(y.x_mid, y.norm2, t->h2, y.rstd2, M, d, mc.rms_eps, s), 1);
+  {  // [gate | up] = h2 * Wgu^T  (no_pre_norms: x_mid * Wgu^T)
     BASEW(W_GU, wgu);
     GemmArgs g;
-    g.A = t->h2; g.lda = d; g.B = wgu; g.ldb = d; g.C = y.gu; g.ldc = 2 * F;
+    g.A = pre_norms ? t->h2 : y.x_mid; g.lda = d; g.B = wgu; g.ldb = d; g.C = y.gu; g.ldc = 2 * F;
     g.M = M; g.N = 2 * F; g.K = d; g.epilogue = EPI_BF16;
     if (fused) {  // silu(gate) * up computed from the accumulator tile ([gate 128 | up 128] interleaved layout)
       g.epilogue = EPI_SWIGLU_FWD; g.aux = t->act; g.ld_aux = F;
@@ -895,6 +905,9 @@ int fwd_bwd(dtx_trainer* t, bool backward) {
       if (rc) return rc;
     }
     Layer& y = t->layers[l];
+    const bool pre_norms = !t->ext.no_pre_norms;  // else the sublayers read xs[l] / x_mid: no norm backward, the residual
+                                                  // gradients are added in the dh2 / dh1 GEMMs' epilogues
+    const bf16* h1 = pre_norms ? y.h1 : t->xs[l];
     const bf16* d_down = cur;  // gradient of the down-projection output
     if (y.pn) {  // through post_mlp_layernorm: d down_pre into dh (free until the dh2 GEMM below); full SFT: its weight gradient
       if (t->full) CK(rmsnorm_dw(cur, y.down_pre, y.rstd_pn2, M, d, t->ndw_scratch, t->grad_of(y.pn + d), accumulate, s), 2);
@@ -916,19 +929,21 @@ int fwd_bwd(dtx_trainer* t, bool backward) {
       CK(gemm_bf16(g, s), 1);
     }
     if (!fused) CK(swiglu_bwd(t->dact, y.gu, t->dgu, M, F, 1, s), 1);
-    {  // dh2 = [dgate | dup] * [Wg ; Wu]
+    {  // dh2 = [dgate | dup] * [Wg ; Wu]  (no_pre_norms: other = d x_mid = d x_next + [dgate | dup] * [Wg ; Wu])
       BASEW(W_GU, wgu);
       GemmArgs g;
       g.A = t->dgu; g.lda = 2 * F; g.B = wgu; g.ldb = d; g.b_mn_major = 1; g.C = t->dh; g.ldc = d;
       g.M = M; g.N = d; g.K = 2 * F; g.epilogue = EPI_BF16;
+      if (!pre_norms) { g.C = other; g.R = cur; g.ldr = d; g.epilogue = EPI_BF16_ADD; }
       CK(gemm_bf16(g, s), 1);
     }
-    if (t->full) {  // dWgu = d[gate|up]^T * h2 (h2 = norm2(x_mid) recomputed) and the norm's own weight gradient
+    if (t->full && !pre_norms) CK(dw_gemm(t->dgu, 2 * F, y.x_mid, d, t->grad_of(y.wgu)), 1);  // dWgu = d[gate|up]^T * x_mid
+    if (t->full && pre_norms) {  // dWgu = d[gate|up]^T * h2 (h2 = norm2(x_mid) recomputed) and the norm's own weight gradient
       CK(rmsnorm_fwd(y.x_mid, y.norm2, t->h2, nullptr, M, d, mc.rms_eps, s), 1);
       CK(dw_gemm(t->dgu, 2 * F, t->h2, d, t->grad_of(y.wgu)), 1);
       CK(rmsnorm_dw(t->dh, y.x_mid, y.rstd2, M, d, t->ndw_scratch, t->grad_of(y.norm2), accumulate, s), 2);
     }
-    CK(rmsnorm_bwd(t->dh, y.x_mid, y.norm2, y.rstd2, cur, other, M, d, s), 1);  // other = d x_mid
+    if (pre_norms) CK(rmsnorm_bwd(t->dh, y.x_mid, y.norm2, y.rstd2, cur, other, M, d, s), 1);  // other = d x_mid
     const bf16* d_o = other;  // gradient of the o-projection output
     if (y.pn) {  // through post_self_attn_layernorm: d o_pre into dh (free until the dh1 GEMM below)
       if (t->full) CK(rmsnorm_dw(other, y.o_pre, y.rstd_pn1, M, d, t->ndw_scratch, t->grad_of(y.pn), accumulate, s), 2);
@@ -965,23 +980,29 @@ int fwd_bwd(dtx_trainer* t, bool backward) {
       CK(qk_norm_bwd(t->dqkv, W, y.qk_pre, QK, M, dq, QK, y.qkn, y.qkn + D, mc.rms_eps, t->full ? t->grad_of(y.qkn) : nullptr,
                      t->ndw_scratch, nblk, accumulate, s), t->full ? 2 : 1);
     }
+    if (y.qkf)  // through OLMo-2's full-width q/k norm, in place; full-parameter SFT: d q_norm | d k_norm
+      CK(qk_norm_full_bwd(t->dqkv, W, y.qk_pre, QK, M, dq, QK, y.qkf, y.qkf + dq, mc.rms_eps, t->full ? t->grad_of(y.qkf) : nullptr,
+                          t->ndw_scratch, accumulate, s), t->full ? 2 : 1);
     if (lora) {  // dt = dqkv * B_ext   [M, RP]
       GemmArgs g;
       g.A = t->dqkv; g.lda = W; g.B = y.b_ext; g.ldb = RP; g.b_mn_major = 1; g.C = t->dt; g.ldc = RP;
       g.M = M; g.N = RP; g.K = W; g.epilogue = EPI_BF16; g.block_n = 64;
       CK(gemm_bf16(g, s), 1);
     }
-    if (t->full) CK(dw_gemm(t->dqkv, W, y.h1, d, t->grad_of(y.wqkv)), 1);  // dWqkv = dqkv^T * h1 (dqkv already carries the inverse rotary)
+    if (t->full) CK(dw_gemm(t->dqkv, W, h1, d, t->grad_of(y.wqkv)), 1);  // dWqkv = dqkv^T * h1 (dqkv already carries the inverse rotary)
     if (t->full && y.bias) CK(bias_grad(t->dqkv, W, M, W, t->grad_of(y.bias), accumulate, s), 1);  // db = column sums of dqkv
     // LoRA: layer 0's input gradient has no consumer (the embedding is frozen, SURVEY §8a): its dh1 GEMM, the dropout-branch
     // gradient and the norm-1 backward are skipped.  Full-parameter SFT trains the embedding and needs them.
     const bool need_dx = l > 0 || t->full;
+    // no_pre_norms: the GEMM writes d x_in = d x_mid + dqkv * Wqkv (+ dt * A_cat) straight into cur, the dropout branch adds to it
+    bf16* dh1 = pre_norms ? t->dh : cur;
     if (need_dx) {  // dh1 = dqkv * Wqkv (+ dt * A_cat in the same accumulator when there is no dropout between h1 and A)
       BASEW(W_QKV, wqkv);
       GemmArgs g;
       g.A = t->dqkv; g.lda = W; g.B = wqkv; g.ldb = d; g.b_mn_major = 1;
       if (lora && !drop) { g.A2 = t->dt; g.lda2 = RP; g.B2 = y.a_cat; g.ldb2 = t->KA; g.K2 = RP; }
-      g.C = t->dh; g.ldc = d; g.M = M; g.N = d; g.K = W; g.epilogue = EPI_BF16;
+      g.C = dh1; g.ldc = d; g.M = M; g.N = d; g.K = W; g.epilogue = EPI_BF16;
+      if (!pre_norms) { g.R = other; g.ldr = d; g.epilogue = EPI_BF16_ADD; }
       CK(gemm_bf16(g, s), 1);
     }
     if (drop && need_dx) {  // dh1 += sum_t mask_t o (dt_t * A_t) / (1 - p): the masks are regenerated from the counter-based RNG
@@ -989,7 +1010,7 @@ int fwd_bwd(dtx_trainer* t, bool backward) {
       g.A = t->dt; g.lda = RP; g.B = y.a_cat; g.ldb = t->KA; g.b_mn_major = 1; g.C = t->glora; g.ldc = t->KA;
       g.M = M; g.N = t->KA; g.K = RP; g.epilogue = EPI_BF16;
       CK(gemm_bf16(g, s), 1);
-      CK(lora_dropout_bwd_add(t->dh, t->glora, M, d, t->nt, p_drop, dropout_key(t, l), s), 1);
+      CK(lora_dropout_bwd_add(dh1, t->glora, M, d, t->nt, p_drop, dropout_key(t, l), s), 1);
     }
     if (lora) {
     {  // grad of B_ext (all rows): dqkv^T * t   [W, RP], split over tokens
@@ -1001,7 +1022,7 @@ int fwd_bwd(dtx_trainer* t, bool backward) {
     }
     {  // grad of A_cat^T: lora_in^T * dt   [KA, RP]
       GemmArgs g;
-      g.A = drop ? y.hd : y.h1; g.lda = t->KA; g.a_mn_major = 1; g.B = t->dt; g.ldb = RP; g.b_mn_major = 1;
+      g.A = drop ? y.hd : h1; g.lda = t->KA; g.a_mn_major = 1; g.B = t->dt; g.ldb = RP; g.b_mn_major = 1;
       g.C = t->part_a; g.ldc = RP; g.M = t->KA; g.N = RP; g.K = M; g.epilogue = EPI_F32; g.split_k = split_a;
       g.block_n = 64;
       CK(gemm_bf16(g, s), 1);
@@ -1019,8 +1040,8 @@ int fwd_bwd(dtx_trainer* t, bool backward) {
       CK(cudaGetLastError(), 2);
     }
     }  // lora
-    if (t->full) CK(rmsnorm_dw(t->dh, t->xs[l], y.rstd1, M, d, t->ndw_scratch, t->grad_of(y.norm1), accumulate, s), 2);
-    if (need_dx) CK(rmsnorm_bwd(t->dh, t->xs[l], y.norm1, y.rstd1, other, cur, M, d, s), 1);  // cur = d x_in
+    if (t->full && pre_norms) CK(rmsnorm_dw(t->dh, t->xs[l], y.rstd1, M, d, t->ndw_scratch, t->grad_of(y.norm1), accumulate, s), 2);
+    if (need_dx && pre_norms) CK(rmsnorm_bwd(t->dh, t->xs[l], y.norm1, y.rstd1, other, cur, M, d, s), 1);  // cur = d x_in
     if (t->full && t->rs_now && t->world > 1) {  // this layer's gradients are final: reduce-scatter them while the backward pass goes on
       int rc = reduce_scatter_block(t, t->g_flat + static_cast<int64_t>(l) * t->layer_elems, t->layer_elems, l);
       if (rc) return rc;
@@ -1579,6 +1600,10 @@ int check_ext(const dtx_model_cfg* mc, const dtx_model_ext* ext) {
   if (ext->rope_glm && ext->qk_norm) return bad("rope_glm cannot be combined with qk_norm");
   if (ext->rope_glm && mc->sliding_window > 0) return bad("rope_glm cannot be combined with a sliding window");
   if (ext->post_norms != 0 && ext->post_norms != 1) return bad("post_norms must be 0 or 1");
+  if (ext->qk_norm_full != 0 && ext->qk_norm_full != 1) return bad("qk_norm_full must be 0 or 1");
+  if (ext->no_pre_norms != 0 && ext->no_pre_norms != 1) return bad("no_pre_norms must be 0 or 1");
+  if (ext->qk_norm_full && (ext->qk_norm || ext->rope_glm)) return bad("qk_norm_full cannot be combined with qk_norm or rope_glm");
+  if (ext->no_pre_norms && !ext->post_norms) return bad("no_pre_norms needs post_norms (the sublayers' only norms)");
   if (ext->rope_glm && ext->rope_type != DTX_ROPE_DEFAULT) return bad("rope_glm needs rope_type DTX_ROPE_DEFAULT (no scaled GLM rotary is implemented)");
   if (ext->rope_type < DTX_ROPE_DEFAULT || ext->rope_type > DTX_ROPE_LLAMA3)
     return bad("rope_type must be DTX_ROPE_DEFAULT, DTX_ROPE_LINEAR or DTX_ROPE_LLAMA3 (yarn, dynamic, longrope are not implemented)");
@@ -1650,8 +1675,10 @@ void setup_dims(dtx_trainer* t, const dtx_model_cfg* mc, const dtx_model_ext* ex
   lname("mlp.up_proj.weight", gu, 0, F, d, GU_UP);
   lname("mlp.gate_up_proj.weight", gu, 0, 2 * F, d, GU_BOTH);  // GLM (modeling_glm GlmMLP: chunk(2))
   lname("mlp.down_proj.weight", lslot(&Layer::wdown, d * F, false, W_DOWN, INIT_NORMAL), 0, d, F);
-  lname("input_layernorm.weight", lslot(&Layer::norm1, d, true, -1, INIT_ONE), 0, d, 1);
-  lname("post_attention_layernorm.weight", lslot(&Layer::norm2, d, true, -1, INIT_ONE), 0, d, 1);
+  if (!t->ext.no_pre_norms) {
+    lname("input_layernorm.weight", lslot(&Layer::norm1, d, true, -1, INIT_ONE), 0, d, 1);
+    lname("post_attention_layernorm.weight", lslot(&Layer::norm2, d, true, -1, INIT_ONE), 0, d, 1);
+  }
   if (t->ext.qkv_bias) {  // Qwen2, GLM: one [W] vector in the row order of wqkv
     const int b = lslot(&Layer::bias, W, true, -1, INIT_ZERO);
     lname("self_attn.q_proj.bias", b, 0, dq, 1);
@@ -1663,10 +1690,16 @@ void setup_dims(dtx_trainer* t, const dtx_model_cfg* mc, const dtx_model_ext* ex
     lname("self_attn.q_norm.weight", q, 0, D, 1);
     lname("self_attn.k_norm.weight", q, D, D, 1);
   }
-  if (t->ext.post_norms) {  // Glm4: post_self_attn_layernorm | post_mlp_layernorm
+  if (t->ext.qk_norm_full) {  // OLMo-2: q_norm [dq] | k_norm [dkv]
+    const int q = lslot(&Layer::qkf, dq + dkv, true, -1, INIT_ONE);
+    lname("self_attn.q_norm.weight", q, 0, dq, 1);
+    lname("self_attn.k_norm.weight", q, dq, dkv, 1);
+  }
+  if (t->ext.post_norms) {  // the norms after the attention and the MLP sublayers, under Glm4's or (no_pre_norms) OLMo-2's names
     const int p = lslot(&Layer::pn, 2 * d, true, -1, INIT_ONE);
-    lname("post_self_attn_layernorm.weight", p, 0, d, 1);
-    lname("post_mlp_layernorm.weight", p, d, d, 1);
+    const bool olmo = t->ext.no_pre_norms;
+    lname(olmo ? "post_attention_layernorm.weight" : "post_self_attn_layernorm.weight", p, 0, d, 1);
+    lname(olmo ? "post_feedforward_layernorm.weight" : "post_mlp_layernorm.weight", p, d, d, 1);
   }
   auto global = [&](bf16* dtx_trainer::*mem, const char* hf, const char* key, int64_t rows, int64_t cols, bool nodecay, int init) {
     t->gnames.push_back({key, hf, static_cast<int>(t->gslots.size()), 0, rows, cols, 0});

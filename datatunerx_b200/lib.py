@@ -44,7 +44,7 @@ class ModelExt(C.Structure):
     _fields_ = [("qkv_bias", C.c_int32), ("rope_type", C.c_int32), ("rope_factor", C.c_float),
                 ("rope_low_freq_factor", C.c_float), ("rope_high_freq_factor", C.c_float), ("rope_original_max_pos", C.c_int32),
                 ("qk_norm", C.c_int32), ("rope_glm", C.c_int32),
-                ("post_norms", C.c_int32)]
+                ("post_norms", C.c_int32), ("qk_norm_full", C.c_int32), ("no_pre_norms", C.c_int32)]
 
 
 class TrainCfg(C.Structure):
@@ -60,7 +60,8 @@ class TrainCfg(C.Structure):
 ABI_SYMBOLS = [
     "dtx_abi_version", "dtx_last_global_error", "dtx_last_error", "dtx_trainer_create", "dtx_trainer_create_ext",
     "dtx_rope_inv_freq", "dtx_plan_device_bytes_ext", "dtx_gemm_bias", "dtx_bias_grad", "dtx_gemm_qk_norm", "dtx_qk_norm_fwd",
-    "dtx_qk_norm_bwd", "dtx_gemm_rope_glm", "dtx_rope_glm_qk", "dtx_attn_bwd_rope", "dtx_post_norm_add", "dtx_trainer_destroy",
+    "dtx_qk_norm_bwd", "dtx_gemm_rope_glm", "dtx_rope_glm_qk", "dtx_attn_bwd_rope", "dtx_post_norm_add", "dtx_qk_norm_full_rope_fwd",
+    "dtx_qk_norm_full_bwd", "dtx_trainer_destroy",
     "dtx_get_nccl_unique_id", "dtx_load_tensor", "dtx_init_random_weights", "dtx_init_lora", "dtx_quantize_base", "dtx_step",
     "dtx_step_device", "dtx_eval_loss", "dtx_allreduce_host", "dtx_export_adapter", "dtx_export_adapter_grad", "dtx_export_weight", "dtx_num_trainable", "dtx_launch_count",
     "dtx_recompute", "dtx_device_bytes", "dtx_plan_device_bytes",
@@ -104,6 +105,8 @@ def load() -> C.CDLL:
     lib.dtx_rope_glm_qk.argtypes = [vp, vp, i32, i32, i32, i32, i32, vp]
     lib.dtx_attn_bwd_rope.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, f32, vp, i32, vp, i32, i32, vp]
     lib.dtx_post_norm_add.argtypes = [vp, vp, vp, vp, vp, i32, i32, C.c_float, vp]
+    lib.dtx_qk_norm_full_rope_fwd.argtypes = [vp, i64, i32, i32, i32, vp, vp, C.c_float, vp, i32, vp, vp, i64, vp]
+    lib.dtx_qk_norm_full_bwd.argtypes = [vp, i64, vp, i64, i32, i32, i32, vp, vp, C.c_float, vp, vp, i32, vp]
     lib.dtx_trainer_destroy.argtypes = [vp]
     lib.dtx_trainer_destroy.restype = None
     lib.dtx_get_nccl_unique_id.argtypes = [vp]
@@ -244,6 +247,11 @@ class ModelConfig:
     # gate_proj | up_proj as one mlp.gate_up_proj tensor, the name weight_names / export_weights use for it
     rope_glm: bool = False
     post_norms: bool = False           # Glm4 post_self_attn_layernorm / post_mlp_layernorm after the two sublayers
+    # OLMo-2 (Olmo2ForCausalLM): q_norm / k_norm over all q / all k columns of a token (weights [n_heads * head_dim] and
+    # [n_kv_heads * head_dim]), and with no_pre_norms (needs post_norms) no input_layernorm / pre-MLP norm: the post-sublayer
+    # norms are then named post_attention_layernorm / post_feedforward_layernorm
+    qk_norm_full: bool = False
+    no_pre_norms: bool = False
     # HF config.json `rope_scaling` / `rope_parameters`: {"rope_type" (or the older "type"): "linear" | "llama3", "factor", ...};
     # None = the plain theta table
     rope_scaling: Optional[dict] = None
@@ -261,11 +269,12 @@ class ModelConfig:
         kind = rs.get("rope_type", rs.get("type", "default"))
         if kind not in ROPE_TYPES:
             raise DtxError(-1, f"rope_type {kind!r}: only {', '.join(ROPE_TYPES)} are implemented natively")
-        qkn, glm, pn = int(bool(self.qk_norm)), int(bool(self.rope_glm)), int(bool(self.post_norms))
+        flags = (int(bool(self.qk_norm)), int(bool(self.rope_glm)), int(bool(self.post_norms)), int(bool(self.qk_norm_full)),
+                 int(bool(self.no_pre_norms)))
         if kind == "default":
-            return ModelExt(int(bool(self.qkv_bias)), 0, 0.0, 0.0, 0.0, 0, qkn, glm, pn)
+            return ModelExt(int(bool(self.qkv_bias)), 0, 0.0, 0.0, 0.0, 0, *flags)
         return ModelExt(int(bool(self.qkv_bias)), ROPE_TYPES[kind], float(rs["factor"]), float(rs.get("low_freq_factor", 0.0)),
-                        float(rs.get("high_freq_factor", 0.0)), int(rs.get("original_max_position_embeddings", 0)), qkn, glm, pn)
+                        float(rs.get("high_freq_factor", 0.0)), int(rs.get("original_max_position_embeddings", 0)), *flags)
 
 
 @dataclass
@@ -452,6 +461,9 @@ class Trainer:
             if m.qk_norm:
                 yield p + "self_attn.q_norm.weight", (m.head_dim,)
                 yield p + "self_attn.k_norm.weight", (m.head_dim,)
+            if m.qk_norm_full:
+                yield p + "self_attn.q_norm.weight", (dq,)
+                yield p + "self_attn.k_norm.weight", (dkv,)
             yield p + "self_attn.o_proj.weight", (d, dq)
             if m.rope_glm:
                 yield p + "mlp.gate_up_proj.weight", (2 * F, d)
@@ -459,6 +471,10 @@ class Trainer:
                 yield p + "mlp.gate_proj.weight", (F, d)
                 yield p + "mlp.up_proj.weight", (F, d)
             yield p + "mlp.down_proj.weight", (d, F)
+            if m.no_pre_norms:
+                yield p + "post_attention_layernorm.weight", (d,)
+                yield p + "post_feedforward_layernorm.weight", (d,)
+                continue
             yield p + "input_layernorm.weight", (d,)
             yield p + "post_attention_layernorm.weight", (d,)
             if m.post_norms:

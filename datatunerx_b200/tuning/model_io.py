@@ -3,7 +3,8 @@
   * load_model_config  : HF config.json -> ModelConfig  (AutoConfig.from_pretrained, cmd/tuning/train.py:221): Llama-2,
                          Llama-3.x (linear / llama3 rope scaling), Mistral, Qwen2 / Qwen2.5 (q/k/v biases), Qwen3 (q/k norm),
                          GLM-4 (GlmForCausalLM / Glm4ForCausalLM: partial interleaved rotary, q/k/v biases,
-                         fused gate_up_proj, Glm4's post-sublayer norms)
+                         fused gate_up_proj, Glm4's post-sublayer norms), OLMo-2 (full-width q/k norm, post-sublayer norms
+                         and no pre-norms)
   * iter_safetensors   : stream tensors of *.safetensors shards (AutoModelForCausalLM.from_pretrained, train.py:236-242);
                          iter_torch_bin does the same for pytorch_model*.bin shards
   * save_peft_adapter  : adapter_config.json + adapter_model.safetensors (+ adapter_model.bin when torch is importable)
@@ -33,17 +34,21 @@ def load_model_config(model_dir: str, full_finetune: bool = False) -> ModelConfi
     """HF config.json -> ModelConfig for the decoders the library trains: Llama-2 / Llama-3.x (`rope_scaling` of type linear or
     llama3), Mistral, Qwen2 / Qwen2.5 (q/k/v biases), Qwen3 (q/k RMSNorm, attention width n_heads * head_dim != hidden) and
     GLM-4 (glm-4-9b-hf, GLM-4-0414, GLM-Z1: GLM's partial interleaved rotary, q/k/v biases from `attention_bias`, and for
-    Glm4ForCausalLM the post-sublayer norms).
+    Glm4ForCausalLM the post-sublayer norms) and OLMo-2 (Olmo2ForCausalLM: q_norm / k_norm over all q / k columns of a token,
+    norms after the two sublayers and none before them).
     Anything that would train a different model than HF's raises ValueError."""
     cfg = json.load(open(os.path.join(model_dir, "config.json")))
     arch = (cfg.get("architectures") or ["LlamaForCausalLM"])[0]
     qwen2, qwen3 = arch == "Qwen2ForCausalLM", arch == "Qwen3ForCausalLM"
     glm4 = arch == "Glm4ForCausalLM"
     glm = arch == "GlmForCausalLM" or glm4
-    if "Llama" not in arch and "Mistral" not in arch and not qwen2 and not qwen3 and not glm:
-        raise ValueError(f"{arch}: only Llama-family, Qwen2, Qwen3 and GLM decoders are implemented natively")
+    olmo2 = arch == "Olmo2ForCausalLM"
+    if "Llama" not in arch and "Mistral" not in arch and not qwen2 and not qwen3 and not glm and not olmo2:
+        raise ValueError(f"{arch}: only Llama-family, Qwen2, Qwen3, GLM and OLMo-2 decoders are implemented natively")
     if glm:
         _check_glm(cfg, full_finetune)
+    elif olmo2:
+        _check_olmo2(cfg, full_finetune)
     elif cfg.get("attention_bias") or cfg.get("mlp_bias"):
         raise ValueError(f"{arch}: attention_bias / mlp_bias are not implemented natively")
     # transformers 5 names the dict `rope_parameters` (it then also carries rope_theta); older configs `rope_scaling`
@@ -71,8 +76,8 @@ def load_model_config(model_dir: str, full_finetune: bool = False) -> ModelConfi
                        n_kv_heads=cfg.get("num_key_value_heads", heads), head_dim=cfg.get("head_dim") or cfg["hidden_size"] // heads,
                        ffn=cfg["intermediate_size"], rms_eps=cfg.get("rms_norm_eps", 1e-5), rope_theta=rope_theta,
                        max_seq=cfg.get("max_position_embeddings", 4096), sliding_window=window,
-                       qkv_bias=qwen2 or (glm and bool(cfg.get("attention_bias", True))), qk_norm=qwen3, rope_glm=glm, post_norms=glm4,
-                       rope_scaling=rs)
+                       qkv_bias=qwen2 or (glm and bool(cfg.get("attention_bias", True))), qk_norm=qwen3, rope_glm=glm,
+                       post_norms=glm4 or olmo2, qk_norm_full=olmo2, no_pre_norms=olmo2, rope_scaling=rs)
 
 
 def _check_glm(cfg: dict, full_finetune: bool) -> None:
@@ -87,6 +92,17 @@ def _check_glm(cfg: dict, full_finetune: bool) -> None:
     if full_finetune and cfg.get("tie_word_embeddings"):
         raise ValueError("full-parameter SFT of a GLM checkpoint with tie_word_embeddings would train the embedding and lm_head as "
                          "two tensors, unlike HF; use LoRA")
+
+
+def _check_olmo2(cfg: dict, full_finetune: bool) -> None:
+    """What Olmo2ForCausalLM may carry and still be the model the library trains (transformers modeling_olmo2)."""
+    if cfg.get("attention_bias"):
+        raise ValueError("OLMo-2 attention_bias is not implemented natively")
+    if cfg.get("hidden_act", "silu") != "silu":
+        raise ValueError(f"OLMo-2 hidden_act {cfg.get('hidden_act')!r}: only silu is implemented natively")
+    if full_finetune and cfg.get("tie_word_embeddings"):
+        raise ValueError("full-parameter SFT of an OLMo-2 checkpoint with tie_word_embeddings would train the embedding and lm_head "
+                         "as two tensors, unlike HF; use LoRA")
 
 
 def check_attention_window(model_dir: str, seq_len: int) -> None:

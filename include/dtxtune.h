@@ -88,9 +88,10 @@ typedef struct {
 } dtx_train_cfg;
 
 /* Model-family extensions of dtx_model_cfg (Llama-3.1 / 3.2 scaled rotary tables, Qwen2 q/k/v projection biases, Qwen3 q/k
- * RMSNorm, GLM's partial interleaved rotary, Glm4's post-sublayer norms).  A NULL or all-zero dtx_model_ext is the plain Llama-2 / Mistral model: no bias,
- * no q/k norm, rotary inverse frequencies theta^(-2i/D) over the whole head.  qk_norm, rope_glm and post_norms were appended after the
- * struct's first release: C callers must be rebuilt against this header (a caller compiled against a shorter struct passes a
+ * RMSNorm, GLM's partial interleaved rotary, Glm4's post-sublayer norms, OLMo-2's full-width q/k RMSNorm and layers without
+ * pre-norms).  A NULL or all-zero dtx_model_ext is the plain Llama-2 / Mistral model: no bias,
+ * no q/k norm, rotary inverse frequencies theta^(-2i/D) over the whole head.  qk_norm, rope_glm, post_norms, qk_norm_full and
+ * no_pre_norms were appended after the struct's first release: C callers must be rebuilt against this header (a caller compiled against a shorter struct passes a
  * struct the library reads past). */
 #define DTX_ROPE_DEFAULT 0   /* inv_freq = theta^(-2i/D) */
 #define DTX_ROPE_LINEAR  1   /* inv_freq / factor (HF rope_type "linear") */
@@ -109,6 +110,12 @@ typedef struct {
   int32_t post_norms;               /* 1: Glm4's post-sublayer norms (Glm4ForCausalLM): post_self_attn_layernorm RMS-normalises
                                        the o_proj output and post_mlp_layernorm the down_proj output before their residual adds
                                        (eps = rms_eps) */
+  int32_t qk_norm_full;             /* 1: OLMo-2's q_norm / k_norm (Olmo2ForCausalLM): one RMSNorm over all n_heads * head_dim q
+                                       columns of a token and one over all n_kv_heads * head_dim k columns (eps = rms_eps),
+                                       before the rotary.  Not with qk_norm or rope_glm */
+  int32_t no_pre_norms;             /* 1: the sublayers read the residual stream itself (OLMo-2: no input_layernorm, no pre-MLP
+                                       norm): x_mid = x + post_norm1(attn(x)), x_next = x_mid + post_norm2(mlp(x_mid)).  Needs
+                                       post_norms */
 } dtx_model_ext;
 
 typedef struct dtx_trainer dtx_trainer;
@@ -125,14 +132,18 @@ DTX_API int32_t dtx_trainer_create(const dtx_model_cfg* model, const dtx_train_c
                            int32_t world, const void* nccl_unique_id, dtx_trainer** out);
 /* The same for a model with family extensions (ext may be NULL: dtx_trainer_create).  An unknown rope_type, a factor <= 0, or
  * for llama3 low_freq_factor >= high_freq_factor or original_max_pos <= 0, or qkv_bias / qk_norm / rope_glm other than 0 / 1,
- * or rope_glm with qk_norm, with a rope_type other than DTX_ROPE_DEFAULT or with a sliding window, or post_norms other than
- * 0 / 1 return DTX_ERR_INVALID before any device work.  With post_norms, "model.layers.N.post_self_attn_layernorm.weight" and
+ * or rope_glm with qk_norm, with a rope_type other than DTX_ROPE_DEFAULT or with a sliding window, or post_norms, qk_norm_full or
+ * no_pre_norms other than 0 / 1, or qk_norm_full with qk_norm or rope_glm, or no_pre_norms without post_norms return
+ * DTX_ERR_INVALID before any device work.  With post_norms, "model.layers.N.post_self_attn_layernorm.weight" and
  * "model.layers.N.post_mlp_layernorm.weight" [hidden] follow the rules of the q/k norm weights below.
  * "model.layers.N.mlp.gate_up_proj.weight" [2 * ffn, hidden] (GLM: gate rows, then up rows) loads in place of gate_proj and
  * up_proj for any model; dtx_export_weight returns it under that name too.
  * With qkv_bias, "model.layers.N.self_attn.{q,k,v}_proj.bias" must be loaded before a step; full-parameter SFT trains them
  * without weight decay (HF get_decay_parameter_names), LoRA keeps them frozen (peft bias="none").  With qk_norm, the same holds
- * for "model.layers.N.self_attn.{q,k}_norm.weight" [head_dim].
+ * for "model.layers.N.self_attn.{q,k}_norm.weight" [head_dim].  With qk_norm_full they are "model.layers.N.self_attn.q_norm.weight"
+ * [n_heads * head_dim] and "...k_norm.weight" [n_kv_heads * head_dim].  With no_pre_norms (OLMo-2 names) the two post-sublayer
+ * norms are "model.layers.N.post_attention_layernorm.weight" and "model.layers.N.post_feedforward_layernorm.weight" [hidden];
+ * such a model has no input_layernorm, and loading one returns DTX_ERR_INVALID (an unknown name).
  * The attention width n_heads * head_dim need not equal hidden (Qwen3, Mistral-Nemo): q_proj is [n_heads * head_dim, hidden],
  * o_proj [hidden, n_heads * head_dim]. */
 DTX_API int32_t dtx_trainer_create_ext(const dtx_model_cfg* model, const dtx_model_ext* ext, const dtx_train_cfg* train,
@@ -319,6 +330,21 @@ DTX_API int32_t dtx_rope_glm_qk(void* qkv, const void* cs_table, int32_t B, int3
  * in fp32; rstd (fp32 [M]) is saved for dtx_rmsnorm_bwd(dy, y, w, rstd, dres = NULL).  out = NULL computes rstd only. */
 DTX_API int32_t dtx_post_norm_add(const void* y, const void* w, const void* res, void* out, void* rstd, int32_t M, int32_t d,
                                   float eps, void* stream);
+/* OLMo-2's full-width q/k RMSNorm and the rotary in one pass, in place on columns [0, n_cols) of a bf16 [M, ld] matrix (the q|k
+ * columns of the plain q|k|v GEMM output): pre (row stride ld_pre) receives the values unchanged, then every row becomes
+ * rotary((x * rsqrt(mean(x^2) + eps)) * w) in fp32, the mean over columns [0, q_cols) with w = wq [q_cols] and over
+ * [q_cols, n_cols) with w = wk [n_cols - q_cols].  The rotary is the half-split one of dtx_gemm_fused's epilogue 3 (pairs i / i + 64
+ * of every 128-column head, cs_table [rope_S][64] from dtx_rope_table); rope_pos (optional device int32 [M]) gives each row's
+ * position, NULL: row % rope_S.  q_cols and n_cols - q_cols: positive multiples of 128, n_cols <= 16384; ld, ld_pre multiples of 8. */
+DTX_API int32_t dtx_qk_norm_full_rope_fwd(void* qkv, int64_t ld, int32_t M, int32_t q_cols, int32_t n_cols, const void* wq,
+                                          const void* wk, float eps, const void* cs_table, int32_t rope_S, const void* rope_pos,
+                                          void* pre, int64_t ld_pre, void* stream);
+/* Its backward, in place on dy (after the inverse rotary): dx = rstd * (w*dy - xh * mean(w*dy*xh)) per span, xh = x * rstd recomputed
+ * from the saved pre-norm x.  dw (optional, bf16 [n_cols]: d q_norm | d k_norm) (+)= sum over rows of dy*xh in a fixed order: 64
+ * blocks of fp32 partials in scratch (>= 64 * n_cols floats, 16-byte aligned), then one more kernel adds them.  accumulate = 0
+ * overwrites dw.  With dw NULL, scratch is ignored. */
+DTX_API int32_t dtx_qk_norm_full_bwd(void* dy, int64_t ld, const void* x, int64_t ldx, int32_t M, int32_t q_cols, int32_t n_cols,
+                                     const void* wq, const void* wk, float eps, void* dw, void* scratch, int32_t accumulate, void* stream);
 DTX_API int32_t dtx_embedding_fwd(const void* ids, const void* table, void* out, int32_t M, int32_t d, int32_t vocab, void* stream);
 DTX_API int32_t dtx_rmsnorm_fwd(const void* x, const void* w, void* y, void* rstd, int32_t M, int32_t d, float eps, void* stream);
 DTX_API int32_t dtx_rmsnorm_bwd(const void* dy, const void* x, const void* w, const void* rstd, const void* dres, void* dx,

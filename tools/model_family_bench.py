@@ -13,6 +13,11 @@
     FFN 13 696, vocab 151 552; q|k|v width 4608), the same workload.  Its q|k|v GEMM (M 8192 x N 4608 x K 4096) with the GLM
     epilogue against the half-split EPI_ROPE epilogue, both with the bias, alternated; post_norm_add at M 8192 x d 4096 (time and
     GB/s); attn_dkv_kernel (torch.profiler) at B 4 x S 2048 with GLM's 32 / 2 heads against Llama-3.1-8B's 32 / 8.
+  * OLMo-2-1124-7B and -13B shapes (full-width q/k norm, post-sublayer norms and no pre-norms, vocab 100 352), the same workload,
+    alternated with the Llama-2-7B shape over `--olmo-rounds` rounds (--olmo); OLMo-2-0325-32B (GQA 40 / 8, FFN 27 648, 64 layers)
+    as QLoRA (NF4 base) at the largest micro-batch of 4, 2, 1 whose bf16 creation-time plan fits in 78 GB; qk_norm_full_rope_fwd
+    and qk_norm_full_bwd (without and with the weight gradient) at M 8192 over the 7B (4096 + 4096) and 32B (5120 + 1024) q|k
+    widths (time and GB/s of the bytes they must move).
 
 The card's name and power limit are read in the same run and printed with the numbers.  Prints one JSON document; --out also
 writes it to a file.
@@ -49,6 +54,13 @@ CONFIGS = {
     "glm-4-9b-0414": L.ModelConfig(vocab=151552, hidden=4096, n_layers=40, n_heads=32, n_kv_heads=2, ffn=13696, rope_theta=10000.0,
                                    max_seq=32768, qkv_bias=True, rope_glm=True, post_norms=True),
 }
+OLMO2 = dict(vocab=100352, rope_theta=500000.0, rms_eps=1e-6, max_seq=4096, qk_norm_full=True, no_pre_norms=True, post_norms=True)
+OLMO_CONFIGS = {
+    "llama2-7b": L.ModelConfig.llama2_7b(),
+    "olmo2-7b": L.ModelConfig(hidden=4096, n_layers=32, n_heads=32, n_kv_heads=32, ffn=11008, **OLMO2),
+    "olmo2-13b": L.ModelConfig(hidden=5120, n_layers=40, n_heads=40, n_kv_heads=40, ffn=13824, **OLMO2),
+}
+OLMO2_32B = L.ModelConfig(hidden=5120, n_layers=64, n_heads=40, n_kv_heads=8, ffn=27648, **OLMO2)
 
 
 def card() -> dict:
@@ -57,11 +69,13 @@ def card() -> dict:
     return {"name": name.strip(), "power_limit": power.strip()}
 
 
-def train_throughput(name: str, mc: L.ModelConfig, B: int, S: int, steps: int, warmup: int, runs: int) -> dict:
+def train_throughput(name: str, mc: L.ModelConfig, B: int, S: int, steps: int, warmup: int, runs: int, quant: bool = False) -> dict:
     tc = L.TrainConfig(micro_batch=B, seq_len=S, total_steps=10 ** 6, lora_r=16, lora_alpha=32.0, lora_dropout=0.0, lr=1e-4)
     planned = {k: L.plan_device_bytes(mc, tc, 1, k) for k in ("keep", "layer")}
     tr = L.Trainer(mc, tc)
     tr.init_random_weights(1234)
+    if quant:
+        tr.quantize_base("int4")
     tr.init_lora(4321)
     batches = [synthetic_batch(s, 0, B, S, mc.vocab) for s in range(4)]
     for s in range(warmup):
@@ -73,7 +87,7 @@ def train_throughput(name: str, mc: L.ModelConfig, B: int, S: int, steps: int, w
             loss, _, _, _ = tr.step(*batches[s % 4])
         rates.append(B * S * steps / (time.perf_counter() - t0))
         losses.append(loss)
-    out = {"config": name, "tokens_per_s_median": statistics.median(rates), "tokens_per_s_range": [min(rates), max(rates)],
+    out = {"config": name + (" qlora-nf4" if quant else ""), "micro_batch": B, "tokens_per_s_median": statistics.median(rates), "tokens_per_s_range": [min(rates), max(rates)],
            "layout": tr.recompute, "planned_bytes": planned, "held_bytes": tr.device_bytes, "last_loss": losses[-1]}
     tr.close()
     return out
@@ -243,6 +257,60 @@ def glm_cost(iters: int, rounds: int) -> dict:
     return res
 
 
+def olmo2_norm_cost(iters: int, rounds: int) -> dict:
+    """qk_norm_full_rope_fwd and qk_norm_full_bwd at M 8192 over OLMo-2-7B's and -32B's q|k widths.  Bytes they must move: the
+    forward reads the q|k columns and writes them twice (pre-norm copy, result in place); the backward reads dy and x and writes dx;
+    with the weight gradient it also writes and reads 64 rows of fp32 partials."""
+    import torch
+    M = 8192
+    lib = L.load()
+    g = torch.Generator().manual_seed(0)
+    stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+    P = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None  # noqa: E731
+    cs = torch.empty(S_ROPE, 64, 2, dtype=torch.float32, device="cuda")
+    L.check(lib.dtx_rope_table(C.c_void_p(cs.data_ptr()), S_ROPE, 128, 500000.0, stream))
+    res = {}
+    for name, dq, dkv in (("7b", 4096, 4096), ("32b", 5120, 1024)):
+        W, QK = dq + 2 * dkv, dq + dkv
+        qkv = (torch.randn(M, W, generator=g) * 0.5).to(torch.bfloat16).cuda()
+        dy = (torch.randn(M, W, generator=g) * 0.1).to(torch.bfloat16).cuda()
+        pre = torch.empty(M, QK, dtype=torch.bfloat16, device="cuda")
+        w = (1 + torch.randn(QK, generator=g) * 0.1).to(torch.bfloat16).cuda()
+        dw = torch.empty(QK, dtype=torch.bfloat16, device="cuda")
+        scratch = torch.empty(64 * QK, dtype=torch.float32, device="cuda")
+        wq, wk = C.c_void_p(w.data_ptr()), C.c_void_p(w.data_ptr() + 2 * dq)
+
+        def launch(v):
+            if v == "fwd":
+                L.check(lib.dtx_qk_norm_full_rope_fwd(P(qkv), W, M, dq, QK, wq, wk, 1e-6, P(cs), S_ROPE, None, P(pre), QK, stream))
+            else:
+                L.check(lib.dtx_qk_norm_full_bwd(P(dy), W, P(pre), QK, M, dq, QK, wq, wk, 1e-6, P(dw) if v == "bwd_dw" else None,
+                                                 P(scratch), 0, stream))
+
+        times = _alternate(launch, ("fwd", "bwd", "bwd_dw"), iters, rounds)
+        out = {"shape": [M, dq, dkv]}
+        for v in ("fwd", "bwd", "bwd_dw"):
+            ms = statistics.median(times[v])
+            nbytes = 3 * M * QK * 2 + (2 * 64 * QK * 4 if v == "bwd_dw" else 0)
+            out[v] = {"ms_median": ms, "ms_range": [min(times[v]), max(times[v])], "bytes": nbytes, "gb_per_s": nbytes / ms / 1e6}
+        res[name] = out
+    return res
+
+
+def olmo2_runs(a) -> dict:
+    """OLMo-2-7B / 13B LoRA alternated with Llama-2-7B; OLMo-2-32B QLoRA"""
+    runs = []
+    for _ in range(a.olmo_rounds):
+        for name, mc in OLMO_CONFIGS.items():
+            runs.append(train_throughput(name, mc, a.batch, a.seq, a.steps, a.warmup, a.runs))
+            print(json.dumps(runs[-1]), flush=True)
+    tc = lambda B: L.TrainConfig(micro_batch=B, seq_len=a.seq, total_steps=1, lora_r=16, lora_dropout=0.0)  # noqa: E731
+    B32 = next((B for B in (4, 2, 1) if L.plan_device_bytes(OLMO2_32B, tc(B), 1, "layer") <= 78e9), 1)
+    runs.append(train_throughput("olmo2-32b", OLMO2_32B, B32, a.seq, max(2, a.steps // 2), a.warmup, a.runs, quant=True))
+    print(json.dumps(runs[-1]), flush=True)
+    return {"runs": runs, "norm_kernels": olmo2_norm_cost(iters=50, rounds=6)}
+
+
 S_ROPE = 2048
 
 
@@ -255,14 +323,19 @@ def main() -> None:
     ap.add_argument("--seq", type=int, default=2048)
     ap.add_argument("--configs", default=",".join(CONFIGS))
     ap.add_argument("--out", default=None)
+    ap.add_argument("--olmo", action="store_true", help="only the OLMo-2 measurements")
+    ap.add_argument("--olmo-rounds", type=int, default=2)
     a = ap.parse_args()
     res = {"card": card(), "lora": "r=16 on q_proj,v_proj", "micro_batch": a.batch, "seq_len": a.seq, "runs": []}
-    for name in a.configs.split(","):
-        res["runs"].append(train_throughput(name, CONFIGS[name], a.batch, a.seq, a.steps, a.warmup, a.runs))
-        print(json.dumps(res["runs"][-1]), flush=True)
-    res["qkv_gemm_bias_cost"] = bias_gemm_cost(iters=50, rounds=6)
-    res["qkv_gemm_qk_norm_cost"] = qk_norm_cost(iters=50, rounds=6)
-    res["glm_cost"] = glm_cost(iters=50, rounds=6)
+    if a.olmo:
+        res["olmo2"] = olmo2_runs(a)
+    else:
+        for name in a.configs.split(","):
+            res["runs"].append(train_throughput(name, CONFIGS[name], a.batch, a.seq, a.steps, a.warmup, a.runs))
+            print(json.dumps(res["runs"][-1]), flush=True)
+        res["qkv_gemm_bias_cost"] = bias_gemm_cost(iters=50, rounds=6)
+        res["qkv_gemm_qk_norm_cost"] = qk_norm_cost(iters=50, rounds=6)
+        res["glm_cost"] = glm_cost(iters=50, rounds=6)
     res["card_after"] = card()
     print(json.dumps(res, indent=1))
     if a.out:
