@@ -27,6 +27,7 @@
 #include "common.cuh"
 #include "kernels.h"
 
+#include <cfloat>
 #include <mutex>
 #include <type_traits>
 
@@ -89,17 +90,18 @@ __device__ __forceinline__ float fast_exp2(float x) {
 
 // 2^x on the FMA pipe (no MUFU): round-to-nearest split x = n + f via the 1.5 * 2^23 trick, cubic minimax for 2^f on
 // [-0.5, 0.5] (max. relative error 7.5e-5, far below bf16 resolution), 2^n added into the exponent field.
-// x is clamped to >= -125 (the polynomial's value can sit just below 1, i.e. in exponent 126, and the exponent field must
-// stay positive after adding n; 2^-125 ~ 0); callers guarantee x <= ~16.
+// The polynomial's argument is clamped to >= -125 (its value can sit just below 1, i.e. in exponent 126, and the exponent field
+// must stay positive after adding n); below the clamp the result is exactly 0, like ex2.approx.ftz's, so that a masked score
+// (-inf) gets weight 0 rather than 2^-125.  Callers guarantee x <= ~16.
 __device__ __forceinline__ float exp2_fma(float x) {
-  x = fmaxf(x, -125.f);
-  const float t = x + 12582912.f;
+  const float xc = fmaxf(x, -125.f);
+  const float t = xc + 12582912.f;
   const float n = t - 12582912.f;
-  const float f = x - n;
+  const float f = xc - n;
   float q = fmaf(0.055171649903059006f, f, 0.2426111251115799f);
   q = fmaf(q, f, 0.6932609677314758f);
   q = fmaf(q, f, 0.9999280571937561f);
-  return __int_as_float(__float_as_int(q) + (__float_as_int(t) << 23));
+  return x < -125.f ? 0.f : __int_as_float(__float_as_int(q) + (__float_as_int(t) << 23));
 }
 // exponential of an element of pair number `pair_idx` of a fragment: every FMA_EVERY-th pair on the FMA pipe (0 = none), the
 // rest on the MUFU
@@ -729,16 +731,34 @@ cudaError_t attn_init_device() {
   if (dev >= 0 && dev < 64) done[dev] = true;
   return cudaSuccess;
 }
+bool aligned16(const void* ptr) { return ptr && (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; }
+
+// The argument rules of AttnArgs, checked on the host before any CUDA call.  Returns the window the kernels run with: a window
+// of S - 1 or more hides no key (query i <= S - 1 sees keys from i - window <= 0), so it runs as plain causal attention (0),
+// which also keeps kv0 + window and friends in the kernels far from int overflow.  -1 = refused.
+int attn_validate(const AttnArgs& a, bool bwd) {
+  if (a.S <= 0 || a.S % 128 || a.B <= 0 || a.H <= 0 || a.Hkv < 0 || a.window < 0) return -1;
+  if (a.H % (a.Hkv > 0 ? a.Hkv : a.H)) return -1;
+  if (!(a.scale > 0.f && a.scale <= FLT_MAX)) return -1;  // the forward's row max commutes with the scaling only for scale > 0
+  if (a.row_start && (a.total_rows <= 0 || a.total_rows % 128)) return -1;
+  if (!aligned16(a.qkv) || !aligned16(a.out)) return -1;  // TMA bases
+  const int window = a.window >= a.S - 1 ? 0 : a.window;
+  if (!bwd) return window;
+  if (!aligned16(a.dout) || !aligned16(a.dqkv) || !aligned16(a.lse) || !aligned16(a.delta)) return -1;
+  // GLM's inverse rotary is instantiated for plain causal attention (GLM has no sliding window)
+  if (a.rope_glm != 0 && (a.rope_glm != 1 || window > 0)) return -1;
+  // the inverse rotary reads the table at freq * rope_stride + pos for pos up to S - 1
+  if (a.rope_cs && a.rope_stride > 0 && a.rope_stride < a.S) return -1;
+  return window;
+}
 }  // namespace
 
 cudaError_t attn_fwd(const AttnArgs& a, cudaStream_t s) {
-  if (a.S % 128 || a.B <= 0 || a.H <= 0) return cudaErrorInvalidValue;
-  if (a.window < 0) return cudaErrorInvalidValue;
+  const int window = attn_validate(a, false);
+  if (window < 0) return cudaErrorInvalidValue;
   cudaError_t e = attn_init_device();
   if (e != cudaSuccess) return e;
   const int Hkv = a.Hkv > 0 ? a.Hkv : a.H;
-  if (a.H % Hkv) return cudaErrorInvalidValue;
-  if (a.row_start && (a.total_rows <= 0 || a.total_rows % 128)) return cudaErrorInvalidValue;
   const uint64_t M = a.row_start ? static_cast<uint64_t>(a.total_rows) : static_cast<uint64_t>(a.B) * a.S, W = static_cast<uint64_t>(a.H + 2 * Hkv) * HD;
   CUtensorMap tmQ, tmKV, tmOut;
   const uint64_t WO = static_cast<uint64_t>(a.H) * HD;
@@ -753,11 +773,11 @@ cudaError_t attn_fwd(const AttnArgs& a, cudaStream_t s) {
   p.lse2 = a.lse;
   p.out = a.out;
   p.seq_lens = a.seq_lens;
-  p.window = a.window;
+  p.window = window;
   p.row_start = a.row_start;
   const int grid = a.B * a.H * (a.S / 128);
 #define DTX_FWD_LAUNCH(E)                                                                          \
-  if (a.window > 0) attn_fwd_kernel<E, true><<<grid, ATT_THREADS, FW_SMEM, s>>>(tmQ, tmKV, tmOut, p); \
+  if (window > 0) attn_fwd_kernel<E, true><<<grid, ATT_THREADS, FW_SMEM, s>>>(tmQ, tmKV, tmOut, p); \
   else attn_fwd_kernel<E, false><<<grid, ATT_THREADS, FW_SMEM, s>>>(tmQ, tmKV, tmOut, p)
   switch (g_fwd_exp_fma_every) {
     case 2: DTX_FWD_LAUNCH(2); break;
@@ -770,15 +790,11 @@ cudaError_t attn_fwd(const AttnArgs& a, cudaStream_t s) {
 }
 
 cudaError_t attn_bwd(const AttnArgs& a, cudaStream_t s) {
-  if (a.S % 128 || a.B <= 0 || a.H <= 0 || !a.delta || !a.lse || !a.dout || !a.dqkv) return cudaErrorInvalidValue;
-  if (a.window < 0) return cudaErrorInvalidValue;
-  // GLM's inverse rotary is instantiated for plain causal attention (GLM has no sliding window)
-  if (a.rope_glm != 0 && (a.rope_glm != 1 || a.window > 0)) return cudaErrorInvalidValue;
+  const int window = attn_validate(a, true);
+  if (window < 0) return cudaErrorInvalidValue;
   cudaError_t e = attn_init_device();
   if (e != cudaSuccess) return e;
   const int Hkv = a.Hkv > 0 ? a.Hkv : a.H;
-  if (a.H % Hkv) return cudaErrorInvalidValue;
-  if (a.row_start && (a.total_rows <= 0 || a.total_rows % 128)) return cudaErrorInvalidValue;
   const uint64_t M = a.row_start ? static_cast<uint64_t>(a.total_rows) : static_cast<uint64_t>(a.B) * a.S, W = static_cast<uint64_t>(a.H + 2 * Hkv) * HD,
                  WO = static_cast<uint64_t>(a.H) * HD;
   CUtensorMap tmQ128, tmKV64, tmDO128, tmDO64, tmDqkv64, tmO128;
@@ -800,10 +816,10 @@ cudaError_t attn_bwd(const AttnArgs& a, cudaStream_t s) {
   p.rope_cs = a.rope_cs;
   p.rope_stride = a.rope_stride > 0 ? a.rope_stride : a.S;
   p.seq_lens = a.seq_lens;
-  p.window = a.window;
+  p.window = window;
   p.row_start = a.row_start;
   const int gq = a.B * a.H * (a.S / 128), gkv = a.B * Hkv * (a.S / 128);
-  const bool win = a.window > 0;
+  const bool win = window > 0;
   if (a.rope_glm && a.rope_cs) {
 #define DTX_DQ_GLM_LAUNCH(I) attn_dq_kernel<false, I, true><<<gq, ATT_THREADS, DQ_SMEM, s>>>(tmQ128, tmKV64, tmDO128, tmO128, tmDqkv64, p)
     if (g_dq_exp_fma_every == 3) DTX_DQ_GLM_LAUNCH(3); else if (g_dq_exp_fma_every == 4) DTX_DQ_GLM_LAUNCH(4); else DTX_DQ_GLM_LAUNCH(0);

@@ -77,13 +77,17 @@ void trainer_set_varlen_split(int on);  // ragged micro-batches run as length gr
 // ---------------------------------------------------------------------------------------------
 // flash attention (causal, head_dim 128), packed qkv layout [B*S, (H + 2*Hkv)*128] (q heads | k heads | v heads per token)
 // ---------------------------------------------------------------------------------------------
+// attn_fwd / attn_bwd return cudaErrorInvalidValue before any CUDA call unless: S > 0 and S % 128 == 0, B > 0, H > 0,
+// Hkv >= 0 and H % Hkv == 0, window >= 0, scale positive and finite, total_rows > 0 and a multiple of 128 with row_start, qkv
+// and out non-null and 16-byte aligned; backward also: dout, dqkv, lse and delta non-null and 16-byte aligned, rope_glm 0 or 1,
+// rope_glm = 1 only without a window, and rope_stride 0 or >= S with rope_cs.  A window >= S - 1 hides no key: it runs as 0.
 struct AttnArgs {
   const bf16* qkv = nullptr;  // [B*S, (H + 2*Hkv)*D]
   bf16* out = nullptr;        // [B*S, H*D]
-  float* lse = nullptr;       // [B, H, S]  natural-log sum-exp of scaled scores
+  float* lse = nullptr;       // [B, H, S]  log2-domain sum-exp of scaled scores (forward: optional)
   int B = 0, S = 0, H = 0;
   int Hkv = 0;                // kv heads; 0 = H (multi-head attention)
-  float scale = 0.f;
+  float scale = 0.f;          // softmax scale (> 0: the forward takes each row's max before scaling)
   // Optional true row lengths (device int32 [B]): rows are right-padded beyond them.  Query / KV tiles that lie entirely in a
   // row's padding are skipped and their outputs (out, dq, dk, dv) written as zeros, the dK/dV kernel stops at the last query
   // block that holds a real token.  nullptr = every row is S long.
@@ -97,7 +101,7 @@ struct AttnArgs {
   const int32_t* row_start = nullptr;
   int total_rows = 0;
   // backward
-  int rope_stride = 0;              // row stride (positions) of the transposed rope table; 0 = S
+  int rope_stride = 0;              // row stride (positions) of the transposed rope table; 0 = S, else >= S
   const float2* rope_cs = nullptr;  // backward only: TRANSPOSED table [64][S] (cos, sin); if set, dq and dk get the inverse rotary applied before the store
   int rope_glm = 0;                 // 1: that inverse rotary is GLM's (partial, interleaved; table [32][S]); needs window 0
   const bf16* dout = nullptr;  // [B*S, H*D]

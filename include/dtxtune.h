@@ -373,16 +373,22 @@ DTX_API int32_t dtx_adamw(void* p, const void* g, void* m, void* v, int64_t n, f
 /* attention: packed qkv [B*S, (H + 2*Hkv)*128]; Hkv < H = grouped-query attention (Mistral / Llama-2-70B).
  *   seq_lens : optional device int32 [B] true row lengths (right padding beyond): tiles entirely in the padding are skipped and
  *              their outputs written as zeros; NULL = all rows full.
- *   window   : sliding-window span (query i sees keys i - window .. i), 0 = plain causal.
+ *   window   : sliding-window span (query i sees keys i - window .. i), 0 = plain causal; any window >= S - 1 is the same as 0.
+ *   scale    : softmax scale, positive and finite.
  *   rope_cs_t (backward): optional TRANSPOSED rotary table [64][rope_stride] float2 - when given, dq and dk leave the kernel
- *              with the inverse rotary applied (what the training step does instead of a separate RoPE-backward kernel). */
+ *              with the inverse rotary applied (what the training step does instead of a separate RoPE-backward kernel);
+ *              rope_stride 0 means S, otherwise it must be >= S.
+ * Both return DTX_ERR_INVALID before any device work unless S > 0 and S % 128 == 0, B > 0, H > 0, Hkv >= 0 (0 = H) and
+ * H % Hkv == 0, window >= 0, the scale is positive and finite, and qkv and out are non-null and 16-byte aligned; the backward
+ * also needs lse2, delta_scratch, dout and dqkv non-null and 16-byte aligned. */
 DTX_API int32_t dtx_attn_fwd(const void* qkv, void* out, void* lse2, int32_t B, int32_t S, int32_t H, int32_t Hkv, float scale,
                      const void* seq_lens, int32_t window, void* stream);
 DTX_API int32_t dtx_attn_bwd(const void* qkv, const void* out, const void* dout, const void* lse2, void* delta_scratch,
                      void* dqkv, int32_t B, int32_t S, int32_t H, int32_t Hkv, float scale, const void* seq_lens,
                      int32_t window, const void* rope_cs_t, int32_t rope_stride, void* stream);
 /* dtx_attn_bwd with a rotary mode for rope_cs_t: rope_glm = 0 is dtx_attn_bwd, 1 applies GLM's inverse rotary (partial,
- * interleaved) from a transposed [32][rope_stride] table; rope_glm = 1 needs window 0. */
+ * interleaved) from a transposed [32][rope_stride] table; rope_glm = 1 needs window 0 (or >= S - 1), other values are
+ * refused.  Without rope_cs_t, rope_glm = 1 runs the plain kernels. */
 DTX_API int32_t dtx_attn_bwd_rope(const void* qkv, const void* out, const void* dout, const void* lse2, void* delta_scratch,
                                   void* dqkv, int32_t B, int32_t S, int32_t H, int32_t Hkv, float scale, const void* seq_lens,
                                   int32_t window, const void* rope_cs_t, int32_t rope_stride, int32_t rope_glm, void* stream);

@@ -74,7 +74,7 @@ def main():
     for every in (3, 0):
         L.set_option("attn_fwd_exp_fma_every", every)
         repeat(f"attn_fwd exp_fma_every={every}", lambda: L.check(lib.dtx_attn_fwd(P(qkv), P(out), P(lse), B, S, H, H, sc, None, 0, ST())), lambda: [out, lse], n=6)
-    L.set_option("attn_fwd_exp_fma_every", 3)
+    L.set_option("attn_fwd_exp_fma_every", 0)
     wo, res = rnd(d, d, scale=0.02, seed=6), rnd(M, d, seed=7)
     xmid = torch.empty(M, d, dtype=torch.bfloat16, device=DEV)
     repeat("o_proj gemm EPI_BF16_ADD", lambda: gemm(out, wo, xmid, R=res, epi=2, m=M, n=d, k=d), lambda: [xmid])
